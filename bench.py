@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- env-steps/s of the packing-environment hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config NAME]          # B200 arm, one JSON line on rank 0
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config NAME] [--dump-outputs DIR]   # GPU arm, one JSON line on rank 0
     python bench.py --impl reference [--gpus N] --steps K --warmup W [--config NAME]   # reference CPU arm (oracle port)
 
 ``--config`` selects one of BASELINE.json's configurations (default ``blockout`` = configs[1], the one the
@@ -28,6 +28,9 @@ Timing: every timed step is bracketed by CUDA events on the launching stream; be
 flushed by writing a 256 MiB buffer (outside the event pairs).  ``value`` uses actions that are already on the
 device; ``e2e`` calls the public ``GpuVecEnv.step`` with HOST actions (pinned H2D copy, kernels, D2H of
 reward/done/info arrays) and is timed with the host clock around the call.
+
+``--dump-outputs DIR`` writes what the last timed step handed its caller (observation, result arrays and, buffered, the
+candidate observation) as ``DIR/<name>.npy`` in float32 / float64; inputs are seeded, so two builds can be compared.
 """
 import argparse
 import json
@@ -50,6 +53,7 @@ BURN_IN = 150            # untimed steps before the W warm-up steps so episodes 
 UNIT = "env-steps/s"
 CPU_ENVS_PER_CORE = 2    # bins per worker process of the CPU arm (same in cpu_baseline and --impl reference)
 CPU_SAMPLES = 3          # the CPU arm reports the median of this many timed samples
+DUMP_LIMIT = 64 * 10 ** 6   # bytes of --dump-outputs; above it a fixed, seeded sample of the bins is written
 DEFAULT_NCCL_CHANNELS = 0   # channels (= SMs) of the rollout all-gather; 0 = NCCL's default (see main_gpu)
 
 CONFIGS = {
@@ -115,6 +119,7 @@ class ClockSampler(object):
         self._stop = threading.Event()
         self.thread = None
         self.how = None
+        self.power_limit_w = None
 
     def _nvml_loop(self, nv, handle):
         masks = [(nv.nvmlClocksEventReasonHwSlowdown, "hw_slowdown"), (nv.nvmlClocksEventReasonHwThermalSlowdown, "hw_thermal_slowdown"),
@@ -136,6 +141,7 @@ class ClockSampler(object):
             # torch numbers the devices like CUDA does; NVML by PCI order: resolve through the UUID-free common case
             # (CUDA_VISIBLE_DEVICES unset, CUDA_DEVICE_ORDER default = fastest first == PCI order on a homogeneous box)
             handle = nv.nvmlDeviceGetHandleByIndex(self.index)
+            self.power_limit_w = nv.nvmlDeviceGetEnforcedPowerLimit(handle) / 1000.0
             self.how = "nvml"
             self.thread = threading.Thread(target=self._nvml_loop, args=(nv, handle), daemon=True)
             self.thread.start()
@@ -180,7 +186,7 @@ class ClockSampler(object):
         for r in self.rows:
             reasons.update(r[2])
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": self.rows[-1][1] if self.rows else None,
-                "reasons": sorted(reasons), "samples": len(sm), "source": self.how}
+                "reasons": sorted(reasons), "samples": len(sm), "source": self.how, "power_limit_w": self.power_limit_w}
 
 
 def device_policy(torch, obs, gen):
@@ -359,8 +365,22 @@ def main_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------------------------------
+
+def dump_outputs(dirname, arrays, n_rows):
+    """Write `arrays` (per-bin NumPy arrays of n_rows rows) as DIR/<name>.npy; when they exceed DUMP_LIMIT only the
+    rows of a fixed, seeded sample of the bins are written, their indices as sample_rows.npy."""
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT:
+        keep = int(DUMP_LIMIT // (total / n_rows + 8))
+        rows = np.sort(np.random.default_rng(0).choice(n_rows, size=keep, replace=False))
+        arrays = {k: v[rows] for k, v in arrays.items()}
+        arrays["sample_rows"] = rows.astype(np.float64)
+    os.makedirs(dirname, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
 
 def overlap_ms(origin, a0, a1, spans):
     """Milliseconds of [a0, a1] that ran concurrently with any of `spans` (pairs of CUDA events);
@@ -423,9 +443,9 @@ def main_gpu(args):
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         # The rollout gather runs beside the next rollout's steps.  NCCL's default all-gather takes up to 32 SMs with
-        # one fat CTA each for its whole duration; the candidates kernel's grid fits the 148 SMs exactly once, so any
-        # SM it loses costs it a second wave (8 GPUs: steps 0.108 -> 0.145 ms while the gather ran).  Fewer channels make
-        # the gather slower but narrower; it has the whole rollout to finish.  IRBPP_NCCL_CHANNELS overrides (0: NCCL's choice).
+        # one fat CTA each for its whole duration; the candidates kernel's grid fills the SM slots, so any SM it loses
+        # can cost it another wave.  Fewer channels make the gather slower but narrower; it has the whole rollout to
+        # finish.  IRBPP_NCCL_CHANNELS overrides (0: NCCL's choice).
         ch = int(os.environ.get("IRBPP_NCCL_CHANNELS", str(DEFAULT_NCCL_CHANNELS)))
         if ch > 0:
             os.environ["NCCL_MAX_NCHANNELS"] = str(ch)
@@ -458,7 +478,7 @@ def main_gpu(args):
         if k > 1:
             if ev is not None:
                 ev[0].record()
-            loc = env.get_action_candidates(choice, as_tensor=True)
+            loc = state["loc"] = env.get_action_candidates(choice, as_tensor=True)
             acts = device_policy(torch, loc, gen)       # the location agent needs the candidates: inside the interval
             state["obs"], _ = env.step_device(acts)
         else:
@@ -482,8 +502,6 @@ def main_gpu(args):
     if world > 1:
         # IRBPP_GATHER: nccl (default: plain all-gather on the side stream) | symm (copy-engine pulls over torch symmetric
         # memory) | compact (all-gather of the packed observations, expanded on arrival) | sendrecv | peer (CUDA IPC pushes).
-        # 8 x B200, 4096 bins each, same box (profiles/README.md): nccl 0.1165 ms/step, compact 0.1212, symm 0.1288 -- the
-        # copy-engine pulls leave the SMs alone but one step beside them took 0.33 ms, the all-gather kernel costs less.
         kind = os.environ.get("IRBPP_GATHER", "nccl")
         gatherer = (sharding.PeerCopyGather(world) if kind == "peer" else sharding.SymmMemGather(world) if kind == "symm" else
                     sharding.CompactRolloutGather(SEL, world) if kind == "compact" and k == 1 else
@@ -532,6 +550,16 @@ def main_gpu(args):
     barrier()
     t_wall = time.perf_counter() - t_wall0
     launches_timed = env.launch_count() - launches0
+    if args.dump_outputs and rank == 0:             # the last timed step's outputs, before any further step replaces them
+        outs = {"obs": state["obs"]}
+        if k > 1:
+            outs["loc_obs"] = state["loc"]
+        res = env.last_step_device()
+        for name in ("reward", "ratio", "ep_reward"):
+            outs[name] = res[name]
+        for name in ("done", "valid", "counter", "ep_len"):
+            outs[name] = res[name].to(torch.float64)
+        dump_outputs(args.dump_outputs, {name: t.cpu().numpy() for name, t in outs.items()}, n_envs)
     # the timed region lasts ~10-30 ms: keep the same loop running (untimed) until nvidia-smi has
     # delivered enough clock samples under this load
     extra_steps = 0
@@ -623,22 +651,10 @@ def main_gpu(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
         bytes_step = algorithmic_bytes_per_env_step(lib, k) * n_envs
         achieved = bytes_step / (kern_ms * 1e-3) / 1e9
-        traffic, traffic_note = None, "no ncu capture of this kernel version / config committed"
-        try:
-            prof = json.load(open(os.path.join(ROOT, "profiles", "step_kernel_traffic.json")))
-            entry = prof.get(args.config)
-            if entry and entry.get("kernel_version") == irbpp_b200.KERNEL_VERSION:
-                traffic = entry.get("dram_bytes_per_launch")
-                traffic_note = "ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum of the step's kernels, %s (%s)" % (
-                    entry.get("source", "profiles/"), entry.get("kernel_version"))
-            elif entry:
-                traffic_note = "committed capture is of kernel version %s, this is %s" % (entry.get("kernel_version"), irbpp_b200.KERNEL_VERSION)
-        except Exception:
-            pass
         line = {"metric": spec["metric"], "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps,
                 "warmup": args.warmup, "ms_per_step": t_dev_ms / args.steps, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
@@ -649,7 +665,7 @@ def main_gpu(args):
                                      + (" + the part of the pipelined rollout all-gather that overlapped neither a timed step nor the agent stand-in" if world > 1 else "")
                                      + ", max over ranks"},
                 "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                             "traffic": traffic, "traffic_note": traffic_note, "peak_source": peak_src,
+                             "peak_source": peak_src,
                              "kernel": "irbpp_scan_kernel + irbpp_candidates_kernel (one step = both launches"
                                        + ("; buffered: a candidates pass + the order-level step" if k > 1 else "") + ")",
                              "kernel_ms": kern_ms, "algorithmic_bytes_per_launch": bytes_step},
@@ -658,7 +674,8 @@ def main_gpu(args):
                         "note": "GpuVecEnv.step(host int64 actions): pinned staging, kernels, reward/done/info arrays back to the "
                                 "host, stream sync; observations stay on the device as in the reference (envs.py:163)"
                                 + ("; includes the exposed part of the rollout all-gather" if world > 1 else "")},
-                "gpu_launches": int(launches_timed), "clocks": clocks, "wall_s_timed_region": t_wall,
+                "gpu_launches": int(launches_timed), "gpu": torch.cuda.get_device_name(dev), "clocks": clocks,
+                "wall_s_timed_region": t_wall,
                 "step_ms": {"median": float(np.median(step_ms)), "min": float(np.min(step_ms)), "max": float(np.max(step_ms))}}
         if world > 1:
             line["gather_ms"] = gather_ms
@@ -688,6 +705,7 @@ def main():
     ap.add_argument("--config", default="blockout", choices=sorted(CONFIGS))
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="bound of the cpu_baseline timed samples (wall seconds, all samples)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * irbpp.h -- C ABI of the B200-native IR-BPP packing-environment hot path.
+ * irbpp.h -- C ABI of the H100-native (sm_90a) IR-BPP packing-environment hot path.
  *
  * The reference (alexfrom0815/IR-BPP) has no FFI layer: its boundary is the Python VecEnv class
  * contract of envs.py:67-165 / wrapper/vec_env.py:29-108 / wrapper/shmem_vec_env.py:20-157.

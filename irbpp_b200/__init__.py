@@ -1,4 +1,4 @@
-"""irbpp_b200: B200-native packing-environment hot path of IR-BPP.
+"""irbpp_b200: H100-native (sm_90a) packing-environment hot path of IR-BPP.
 
 Submodules (imported lazily so CPU-only tooling can use ``shapes`` without the
 CUDA library): ``shapes`` (shape tables), ``_lib`` (ctypes binding of the C-ABI

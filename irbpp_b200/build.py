@@ -1,4 +1,4 @@
-"""Build the CUDA library (in-tree, sm_100a only).  ``python -m irbpp_b200.build``"""
+"""Build the CUDA library (in-tree, sm_90a only).  ``python -m irbpp_b200.build``"""
 import os
 import subprocess
 import sys
@@ -15,7 +15,7 @@ OUT = os.path.join(OUT_DIR, "libirbpp.so")
 # experiment hook: extra -D flags and an alternative output name (IRBPP_LIB selects it at load time)
 EXTRA_DEFS = os.environ.get("IRBPP_BUILD_DEFS", "").split()
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-fmad=false",                      # float64 must round exactly like NumPy: no FMA contraction
               "-Xcompiler", "-fPIC", "-shared"]
 

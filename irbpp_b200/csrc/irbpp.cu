@@ -527,7 +527,7 @@ static int step_async_impl(irbpp_env* h, const int64_t* actions, int32_t on_devi
         P.actions = actions;
         rc = launch(h, P, s); if (rc) return rc;
     } else {
-        // host actions: pinned staging + one H2D copy (measured 12 us faster end to end than letting the kernel read
+        // host actions: pinned staging + one H2D copy (measured faster end to end than letting the kernel read
         // them over PCIe); results: every bin's thread 0 also stores them into this step's pinned host block
         memcpy(h->actions_pinned, actions, (size_t)P.N * sizeof(int64_t));
         P.actions = h->actions_dev;
@@ -544,7 +544,7 @@ static int step_async_impl(irbpp_env* h, const int64_t* actions, int32_t on_devi
         P.h_valid = reinterpret_cast<uint8_t*>(b); b += N;
         P.h_error = reinterpret_cast<uint8_t*>(b);
         // (One CUDA graph per step -- H2D copy + both kernels, instantiated per observation buffer -- was measured:
-        // submit 12.8 -> 8.8 us, but the step's wait grew by as much, e2e 0.162 vs 0.155 ms; dropped.)
+        // a shorter submit, but the step's wait grew by as much; dropped.)
         CUDA_TRY(h, cudaMemcpyAsync(h->actions_dev, h->actions_pinned, (size_t)P.N * sizeof(int64_t), cudaMemcpyHostToDevice, s));
         rc = launch(h, P, s); if (rc) return rc;
     }
@@ -809,6 +809,13 @@ int irbpp_unpack_observations(const void* packed, int32_t selected_action, int32
 }
 
 // ---- point clouds of the next items (SURVEY.md 8(f)3; csrc/irbpp_pointnet.cuh) ----------------------------------
+// grid of the grid-stride gather kernels: 16 CTAs per SM of the device that runs them
+static int64_t gather_grid_cap(int dev) {
+    int sms = 0;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 1;
+    return (int64_t)sms * 16;
+}
+
 static int pn_common(PointNetParams& Q, const float* shape_array, int32_t S, int32_t P, const float* obs, int64_t obs_stride,
                      int32_t item_col, const int32_t* ids, int32_t B, uint64_t seed, uint64_t counter, int32_t n_points) {
     if (!shape_array || S <= 0 || P <= 0 || B <= 0 || n_points <= 0) return fail(nullptr, IRBPP_EINVAL, "bad point-cloud arguments");
@@ -827,9 +834,10 @@ int irbpp_sample_point_clouds(const float* shape_array, int32_t S, int32_t P, co
     int rc = pn_common(Q, shape_array, S, P, obs, obs_stride, item_col, ids, B, seed, counter, n_points); if (rc) return rc;
     if (!out) return fail(nullptr, IRBPP_EINVAL, "null output");
     Q.out = out; Q.indices_out = indices_out;
-    DeviceGuard guard(device_of(shape_array));
+    const int dev = device_of(shape_array);
+    DeviceGuard guard(dev);
     const int64_t n = (int64_t)B * n_points;
-    const int blocks = (int)std::min<int64_t>((n + 255) / 256, 148 * 16);
+    const int blocks = (int)std::min<int64_t>((n + 255) / 256, gather_grid_cap(dev));
     irbpp_cloud_gather_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(Q);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "kernel launch: %s", cudaGetErrorString(e));
@@ -853,7 +861,7 @@ int irbpp_shape_features(const float* shape_array, int32_t S, int32_t P, const f
     const int tiles = (n_points + PN_TILE - 1) / PN_TILE;
     irbpp_shape_encode_kernel<<<S * tiles, PN_THREADS, PN_SMEM_BYTES, s>>>(Q);
     const int64_t n = (int64_t)B * PN_H;
-    irbpp_feature_gather_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 148 * 16), 256, 0, s>>>(Q);
+    irbpp_feature_gather_kernel<<<(int)std::min<int64_t>((n + 255) / 256, gather_grid_cap(dev)), 256, 0, s>>>(Q);
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "kernel launch: %s", cudaGetErrorString(e));
     return IRBPP_OK;

@@ -205,7 +205,7 @@ __device__ void finish_polygon(S& sc, int n, int pos, Emit emit) {
 // (callers pass d = (1, 0), hi = 0 for "squared distance to the point a": the seeding rounds and degenerate
 // segments).  Four positions per trip: their loads and products are independent, only the final compare chain is
 // ordered, so a lane's dependent chain per four points is about as long as it used to be per point -- the chain,
-// not the instruction count, is what the lock-stepped warp waits for (profiles/).
+// not the instruction count, is what the lock-stepped warp waits for.
 template <class S>
 __device__ __forceinline__ void farthest_on_arc(const S& sc, int n, int s, int len, int ax, int ay, int dx, int dy, int hi,
                                                 bool legacy, int& best, int& bi) {

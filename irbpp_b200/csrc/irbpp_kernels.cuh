@@ -1,4 +1,4 @@
-// irbpp_kernels.cuh -- the packing-environment step as two kernels for sm_100a.
+// irbpp_kernels.cuh -- the packing-environment step as two kernels for sm_90a.
 //
 //   irbpp_scan_kernel        one CTA (128 threads) per bin
 //     A  apply the chosen candidate: decode (binPhy.py:234-236), prejudge (:238-245), drop height of that
@@ -23,10 +23,10 @@
 // (paths relative to the reference root)
 //
 // Why two kernels: phase C is one serial task per lane with ~40 tasks per bin; inside a one-bin CTA it
-// ran at ~3 active lanes per instruction and left the other warps waiting at a barrier (profiles/).
+// ran at ~3 active lanes per instruction and left the other warps waiting at a barrier.
 // Splitting lets phase C pack tasks of several bins into full warps and lets phase B run with 12 KB of
 // shared memory per CTA.  The hand-over (float64 drop heights, masks, level bitmaps: ~9 KB per bin) is
-// written and re-read within microseconds and stays in the 126 MB L2.
+// written and re-read within microseconds and stays in L2 (37 MB for 4096 bins; the H100 has 50 MB).
 //
 // Arithmetic is IEEE float64 exactly as NumPy performs it (compile with -fmad=false); masks are
 // folded into the tables as +/-inf sentinels at load time, which changes no comparison result.
@@ -47,9 +47,9 @@ constexpr int NPOSE = AX * AY;           // 256 poses per rotation
 constexpr int CTA_THREADS = 128;
 constexpr int CTA_WARPS = CTA_THREADS / 32;
 // CTA shapes of the candidates kernel (one warp per bin): 4 bins per CTA up to four rotations, 8 from WIDE_MIN_R rotations on.
-// Measured (profiles/README.md, round 2 sweep): BlockOut R = 4  0.109 ms with 4 bins / 0.126 with 8 (512 CTAs of 62 KB no longer
-// fit one wave); irregular R = 8  0.370 / 0.355; R = 24  2.91 / 2.28 -- with many rotations a CTA's fixed phases amortise over
-// more images and the task deal balances over 256 lanes.  Fewer than 4 bins, or more warps than bins, lost everywhere.
+// Measured on an H100 SXM (700 W), ms per step of 4096 bins: BlockOut R = 4  0.147 with 4 bins / 0.158 with 8 (three 62 KB CTAs per SM:
+// 512 of them take two waves); irregular R = 8 and R = 24 within noise with 6, 7 or 8 (0.373-0.379, 2.55-2.57) -- with many
+// rotations a CTA's fixed phases amortise over more images and the task deal balances over 256 lanes.
 #ifndef IRBPP_ENVS_PER_CTA
 #define IRBPP_ENVS_PER_CTA 4
 #endif
@@ -416,7 +416,7 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
 
 // ---- scan -> candidates hand-over flags -------------------------------------------------------------------
 // The candidates grid is launched programmatically (PDL) and becomes resident while the scan grid's last wave
-// drains (3.46 waves on the bench workload: for ~13 us about half the SM slots have no scan CTA).  Waiting there
+// drains (on the bench workload the scan grid is several waves; in the last one SM slots fall idle).  Waiting there
 // for the WHOLE scan grid (griddepcontrol.wait) wastes that time for every bin of an earlier wave, so a scan CTA
 // publishes a per-unit flag (release) once its part of the scratch is written and a candidates CTA starts as soon
 // as the flags of ITS bins carry this launch's epoch (acquire).  No deadlock: the scan CTAs trigger the dependent
@@ -863,7 +863,7 @@ static_assert(RANK_BUCKETS % 32 == 0 && 32 * ROWS_WORDS >= 2 * RANK_BUCKETS, "ph
 // every pose of the bin (4 KB).  Beyond that a worst-case sized scratch would decide the residency (8 KB per warp at R = 8:
 // 4 CTAs per SM in two waves, 12.7 warps active; 24 KB at R = 24: 2 CTAs), so the scratch stays at 4 KB, a bin whose
 // candidates fit it (Ktot <= 1024, the usual case at R = 8) keeps its lists there and only a larger one spills to a global
-// scratch (Params::dlist, L2 resident).  Measured: irregular R = 8  0.390 -> 0.370 ms per step, R = 24 unchanged.
+// scratch (Params::dlist, L2 resident).
 #ifndef IRBPP_LISTS_SMEM_MAX_R
 #define IRBPP_LISTS_SMEM_MAX_R 4
 #endif
@@ -1077,8 +1077,7 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
         // 2. micro-tasks: one (image, start pixel) pair each, TASKS_PER_LANE per lane and batch.  The tasks are in cost
         //    order, so task slot 0 of the lanes holds the 128 most expensive ones (64-point scratch), slots 1 and 2 the
         //    cheap rest (32-point scratch): one follow / sort / approximate cycle with its five block barriers serves
-        //    up to 384 tasks -- a 4-bin CTA of the bench workload has ~170 (profiles/: per-CTA timelines showed the
-        //    second and third cycle of the one-task-per-lane form costing 7.5 us of a 43 us CTA, 30 us in the worst)
+        //    up to 384 tasks -- a 4-bin CTA of the bench workload has ~170
         constexpr int TPL = TASKS_PER_LANE;
         constexpr int BATCH = CAND_THREADS * TPL;
         static_assert(FAST_CAP * 32 + (TPL - 1) * 32 * 32 <= WS_MIN_BYTES, "the task slots' point buffers share the warp scratch");

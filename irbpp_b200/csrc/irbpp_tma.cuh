@@ -1,5 +1,5 @@
 // irbpp_tma.cuh -- 1-D bulk asynchronous copies (the TMA engine's cp.async.bulk) global -> shared memory with
-// an mbarrier as completion object, for sm_100a.  One elected thread arms the barrier with the byte count and
+// an mbarrier as completion object, for sm_90a.  One elected thread arms the barrier with the byte count and
 // issues the copies; the data is moved by the copy engine, not through registers; consumers wait on the
 // barrier's phase parity.  Sizes and both addresses must be multiples of 16 bytes.
 // Under the test-only host emulation (tests/host_harness/cuda_emu.h defines IRBPP_HOST_EMULATION) the copy is a

@@ -136,8 +136,8 @@ class AsyncRolloutGather(object):
 class CompactRolloutGather(object):
     """AsyncRolloutGather over the compact form of the location observation (``csrc/irbpp_pack.cuh``: 7 184 instead of
     14 132 bytes per bin at selectedAction = 500, lossless): pack on the sender, all-gather the packed rows, expand on the
-    receiver.  The gather's duration -- and with it the stretch of steps it disturbs -- halves; the two extra kernels
-    cost ~0.02 ms (pack, 4096 bins) and ~0.1 ms (expanding 8 x 4096 bins).  CUDA tensors only (the kernels are in libirbpp)."""
+    receiver.  The gather's duration -- and with it the stretch of steps it disturbs -- halves, at the cost of the two
+    extra kernels.  CUDA tensors only (the kernels are in libirbpp)."""
 
     def __init__(self, selected_action, world_size=None, group=None):
         import ctypes
@@ -198,7 +198,7 @@ class PeerCopyGather(object):
     shard straight into every peer's gathered buffer over NVLink (the buffers are exchanged once as CUDA IPC handles),
     then a 4-byte NCCL all-reduce on the same side stream tells each rank that all pushes into ITS buffer are done.
     An NCCL all-gather occupies SMs on every GPU for its whole duration, and beside the latency-bound step kernels
-    it cost almost as much step time as it took itself (8 GPUs: steps 0.108 -> 0.145 ms while a 0.78 ms gather ran);
+    it cost almost as much step time as it took itself;
     copy-engine traffic does not compete for SMs, so it really runs beside the next rollout's steps.
     Same interface as AsyncRolloutGather; a gathered buffer stays valid until the second next ``start``.
     One node only (CUDA IPC); falls back to AsyncRolloutGather if the handles cannot be exchanged."""

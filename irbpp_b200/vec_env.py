@@ -173,7 +173,7 @@ def _as_host_i64(a, n, what):
 
 
 class GpuVecEnv(VecEnv):
-    """N packing bins resident on one B200 behind the VecEnv contract.
+    """N packing bins resident on one GPU behind the VecEnv contract.
 
     Parameters mirror what ``PackingGame.__init__`` reads from ``args`` (binPhy.py:25-49):
     ``library`` is a ``shapes.ShapeLibrary`` (the ``shotInfo`` / ``shapeDict`` / ``infoDict`` data),

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
     if not config.pluginmanager.hasplugin("timeout"):
         # pytest-timeout absent: the marker is registered so that it is not an unknown-mark warning, and the emulated
         # kernel tests (which rely on it against deadlocked barriers) install their own watchdog (see below)

@@ -159,6 +159,7 @@ typedef void* cudaStream_t;
 enum cudaMemcpyKind { cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice };
 constexpr unsigned cudaHostAllocMapped = 2;
 enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize };
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount };
 enum cudaLaunchAttributeID { cudaLaunchAttributeProgrammaticStreamSerialization };
 struct cudaLaunchAttribute { cudaLaunchAttributeID id; struct { int programmaticStreamSerializationAllowed; } val; };
 struct cudaLaunchConfig_t { dim3 gridDim, blockDim; size_t dynamicSmemBytes; cudaStream_t stream; cudaLaunchAttribute* attrs; unsigned numAttrs; };
@@ -167,6 +168,7 @@ static inline const char* cudaGetErrorString(cudaError_t) { return "emulated"; }
 static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 static inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
+static inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr, int) { *v = 1; return cudaSuccess; }
 static inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
 static inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return cudaSuccess; }
 static inline cudaError_t cudaGetLastError() { return cudaSuccess; }

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: ``pytest -m gpu``).  Every check goes through the C ABI
+"""GPU parity tests (run on an H100: ``pytest -m gpu``).  Every check goes through the C ABI
 (ctypes -> libirbpp.so -> irbpp_scan_kernel / irbpp_candidates_kernel) and compares with (a) the committed outputs of the
 UNMODIFIED reference (tests/golden) and (b) the oracle on the same seeded inputs.  Bar: value-exact
 (``np.array_equal``; -0.0 == +0.0, SURVEY.md 8c) for every float64 view and for the float32

@@ -3,7 +3,7 @@ thread per CUDA thread of one block at a time, real barriers, warp collectives a
 compared with the golden episodes of the unmodified reference.  TEST INFRASTRUCTURE ONLY: it checks the
 kernel-level logic (barrier structure, hand-overs, warp collectives) where no GPU exists; the emulated
 library exports ``emu_irbpp_*`` symbols, which ``irbpp_b200._lib`` cannot bind, and lives in a temp dir.
-The parity tests proper are the ``-m gpu`` tests, which run the real kernels on a B200."""
+The parity tests proper are the ``-m gpu`` tests, which run the real kernels on an H100."""
 import ctypes
 import os
 import re

@@ -1,5 +1,5 @@
-"""Key metrics of every kernel in an ncu report (the table committed under profiles/).
-    python tools/ncu_summary.py gpurun_out/prof14.ncu-rep > profiles/r01_v14_ncu_summary.txt
+"""Key metrics of every kernel in an ncu report.
+    python tools/ncu_summary.py prof.ncu-rep > ncu_summary.txt
 """
 import csv
 import io
