@@ -194,12 +194,8 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     P.resZ = cfg->resolution_z;
     P.resA = cfg->resolution_act;
     P.binvol = (cfg->bin_dimension[0] * cfg->bin_dimension[1]) * cfg->bin_dimension[2];   // np.prod
-    P.ws_bytes = ws_bytes_for(P.R);
     h->epc = envs_per_cta_for(P.R);                  // bins (= warps) per CTA of the candidates kernel
-    {
-        const size_t fixed = h->epc == ENVS_PER_CTA_WIDE ? sizeof(CandSmem<ENVS_PER_CTA_WIDE>) : sizeof(CandSmem<ENVS_PER_CTA_NARROW>);
-        h->cand_smem = (int)((fixed + 15) & ~(size_t)15) + h->epc * P.ws_bytes + h->epc * P.R * 8 * 4;
-    }
+    h->cand_smem = h->epc == ENVS_PER_CTA_WIDE ? cand_smem_bytes<ENVS_PER_CTA_WIDE>(P.R) : cand_smem_bytes<ENVS_PER_CTA_NARROW>(P.R);
 
 #define TRY_ALLOC(expr)                                                                          \
     do { cudaError_t e2_ = (expr); if (e2_ != cudaSuccess) {                                      \
@@ -216,7 +212,7 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     TRY_ALLOC(dev_alloc(h, &P.maskbits, units * P.R * 8));
     TRY_ALLOC(dev_alloc(h, &P.bitmaps, units * P.R * MAX_LEVELS * 8));
     TRY_ALLOC(dev_alloc(h, &P.nlevels, units * P.R));
-    if (!lists_in_smem(P.R)) TRY_ALLOC(dev_alloc(h, &P.dlist, units * 2 * P.R * NPOSE));
+    if (P.R * NPOSE > LIST_CAP_WS) TRY_ALLOC(dev_alloc(h, &P.dlist, units * 2 * P.R * NPOSE));     // phase-D lists of bins that spill
     TRY_ALLOC(dev_alloc(h, &h->ready_dev, units));        // zeroed: no launch has epoch 0
     // result block (8-byte fields first so every array stays aligned)
     h->results_bytes = (size_t)N * (8 + 8 + 4 + 4 + 4 + 1 + 1 + 1);

@@ -11,7 +11,7 @@
 //        floor_divide semantics (cvTools.py:78-79); one 16x16 bitmap per (rotation, level) by warp
 //        ballots -> global scratch (L2 resident).  Tables that are constant on square blocks of cells
 //        (voxel shapes) are scanned from block maxima of the heightmap (TileEntry lists)
-//   irbpp_candidates_kernel  one CTA per 4 bins (up to four rotations) or 8 bins (from R = 8), one warp per bin
+//   irbpp_candidates_kernel  one CTA per 4 bins (up to seven rotations) or 8 bins (from R = 8), one warp per bin
 //     C  candidate extraction (cvTools.py:61-103): the (bin, rotation, level) images of the CTA are
 //        ordered by a cost key; every (image, start pixel) pair is one lane's task, dealt in that order
 //        so that the lanes of a warp carry contours of similar length: border following, then (after
@@ -46,10 +46,11 @@ constexpr int STEP = 2;                  // stepSize = resolutionAct / resolutio
 constexpr int NPOSE = AX * AY;           // 256 poses per rotation
 constexpr int CTA_THREADS = 128;
 constexpr int CTA_WARPS = CTA_THREADS / 32;
-// CTA shapes of the candidates kernel (one warp per bin): 4 bins per CTA up to four rotations, 8 from WIDE_MIN_R rotations on.
-// Measured on an H100 SXM (700 W), ms per step of 4096 bins: BlockOut R = 4  0.147 with 4 bins / 0.158 with 8 (three 62 KB CTAs per SM:
-// 512 of them take two waves); irregular R = 8 and R = 24 within noise with 6, 7 or 8 (0.373-0.379, 2.55-2.57) -- with many
-// rotations a CTA's fixed phases amortise over more images and the task deal balances over 256 lanes.
+// CTA shapes of the candidates kernel (one warp per bin): 4 bins per CTA below WIDE_MIN_R rotations, 8 from there on.  Both are
+// built for 32 warps per SM (cand_min_ctas), so the 1024 / 512 CTAs of a 4096-bin step run in one wave on 132 SMs.
+// Timed on an H100 SXM (700 W) with the earlier 4 KB warp scratch, ms per step of 4096 bins: BlockOut R = 4  0.147 with 4 bins /
+// 0.158 with 8; irregular R = 8 and R = 24 within noise with 6, 7 or 8 (0.373-0.379, 2.55-2.57) -- with many rotations a CTA's
+// fixed phases amortise over more images and the task deal balances over 256 lanes.
 #ifndef IRBPP_ENVS_PER_CTA
 #define IRBPP_ENVS_PER_CTA 4
 #endif
@@ -64,7 +65,7 @@ constexpr int ENVS_PER_CTA_WIDE = IRBPP_ENVS_PER_CTA_WIDE;
 __host__ __device__ inline int envs_per_cta_for(int R) { return R >= IRBPP_WIDE_MIN_R ? ENVS_PER_CTA_WIDE : ENVS_PER_CTA_NARROW; }
 constexpr int MAX_LEVELS = 64;           // level-image slots per (bin, rotation) in the scratch
 #ifndef IRBPP_TASKS_PER_LANE
-#define IRBPP_TASKS_PER_LANE 3
+#define IRBPP_TASKS_PER_LANE 2
 #endif
 constexpr int TASKS_PER_LANE = IRBPP_TASKS_PER_LANE;        // micro-tasks a lane takes per batch of the candidates kernel (one follow / sort / approximate cycle)
 constexpr int TASK_TAB = 384;            // start pixels of a round listed explicitly (the rest are found by search)
@@ -159,8 +160,7 @@ struct Params {
     const int64_t* actions;              // MODE_STEP / MODE_CANDIDATES
     const uint8_t* which;                // MODE_RESET (NULL = all)
     const int32_t* dbg_items;            // MODE_DEBUG_SCAN
-    int32_t ws_bytes;                    // per-warp scratch of the candidates kernel (ws_bytes_for(R))
-    uint16_t* dlist;                     // [units][2][R*256] phase D lists for R > LISTS_SMEM_MAX_R, else NULL
+    uint16_t* dlist;                     // [units][2][R*256] phase D lists of bins with more than LIST_CAP_WS candidates (NULL if R*256 <= LIST_CAP_WS)
     uint32_t* ready;                     // [units] hand-over flags: the scan CTA of a unit stores `epoch` when its scratch is written (NULL: grid-wide wait)
     uint32_t epoch;                      // value of this launch (never 0)
     int32_t pose_actions;                // MODE_STEP: actions are flat poses (rot*256 + lx*16 + ly), not candidate rows
@@ -851,28 +851,21 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
 // that the lanes of a warp carry images of similar size -- the lanes run in lock step and a warp costs
 // what its heaviest lane costs (the floor-level image of each rotation is an order of magnitude
 // heavier than the small plateaus above it).
-// Per-warp scratch of the candidates kernel, sized at run time (Params::ws_bytes, >= WS_MIN_BYTES): the first
-// FAST_CAP * 32 bytes are the lane-strided contour points of phase C (also the 1024-point overflow
-// buffers); in phase D the whole block holds the candidate list and its bucket-sorted index list, so its
-// size grows with the rotation count (a bin can have up to R * 256 candidates).
-constexpr int WS_MIN_BYTES = 4096;
-static_assert(WS_MIN_BYTES >= 2 * BIG_CAP && WS_MIN_BYTES >= FAST_CAP * 32, "overflow buffers must fit the lane scratch");
+// Per-warp scratch of the candidates kernel, 3 KB for every rotation count: in phase C the lane-strided contour points of
+// the task slots (FAST_CAP points for slot 0, SLOT_CAP for the others) and the 1024-point overflow buffers; in phase D the
+// candidate list + its bucket-sorted entry list (2 x uint16 per candidate).  A bin with more than LIST_CAP_WS candidates
+// (BlockOut bins of the bench workload have at most ~210 of the 1024 possible at R = 4) spills its lists to a global
+// scratch (Params::dlist, L2 resident).  A scratch sized for the worst case would decide the residency instead (4 KB per
+// warp at R = 4 left seven 4-bin CTAs per SM: 924 on 132 SMs, so 4096 bins took a second wave).
+constexpr int WS_BYTES = 3072;
+constexpr int LIST_CAP_WS = WS_BYTES / 4;                // candidates whose lists fit the warp scratch
+constexpr int SLOT_CAP_FIT = TASKS_PER_LANE > 1 ? (WS_BYTES - FAST_CAP * 32) / ((TASKS_PER_LANE - 1) * 32) : FAST_CAP;
+constexpr int SLOT_CAP = SLOT_CAP_FIT < FAST_CAP ? SLOT_CAP_FIT : FAST_CAP;     // contour points of task slots 1.. (slot 0: FAST_CAP)
+static_assert(WS_BYTES % 16 == 0 && WS_BYTES >= 2 * BIG_CAP, "the serial overflow redo lays two 1024-point buffers over the warp scratch");
+static_assert(SLOT_CAP >= 16 && FAST_CAP * 32 + (TASKS_PER_LANE - 1) * SLOT_CAP * 32 <= WS_BYTES,
+              "the task slots' point buffers share the warp scratch");
 constexpr int RANK_BUCKETS = 256;                        // height buckets of the phase-D truncation ranking (per warp: bases + cursors)
 static_assert(RANK_BUCKETS % 32 == 0 && 32 * ROWS_WORDS >= 2 * RANK_BUCKETS, "phase D's rank histograms reuse the image slots (one warp's share each)");
-// Phase D's candidate list + bucket-sorted entry list (2 x uint16 per candidate): up to R = 4 the warp scratch holds them for
-// every pose of the bin (4 KB).  Beyond that a worst-case sized scratch would decide the residency (8 KB per warp at R = 8:
-// 4 CTAs per SM in two waves, 12.7 warps active; 24 KB at R = 24: 2 CTAs), so the scratch stays at 4 KB, a bin whose
-// candidates fit it (Ktot <= 1024, the usual case at R = 8) keeps its lists there and only a larger one spills to a global
-// scratch (Params::dlist, L2 resident).
-#ifndef IRBPP_LISTS_SMEM_MAX_R
-#define IRBPP_LISTS_SMEM_MAX_R 4
-#endif
-constexpr int LISTS_SMEM_MAX_R = IRBPP_LISTS_SMEM_MAX_R;
-__host__ __device__ inline bool lists_in_smem(int R) { return R <= LISTS_SMEM_MAX_R; }
-__host__ __device__ inline int ws_bytes_for(int R) {
-    const int need = lists_in_smem(R) ? R * NPOSE * 4 : 0;     // uint16 list + uint16 sorted list for every pose
-    return ((need > WS_MIN_BYTES ? need : WS_MIN_BYTES) + 15) & ~15;
-}
 
 template <int EPC>
 struct CandSmem {
@@ -891,8 +884,24 @@ struct CandSmem {
     int32_t error[ENVS_PER_CTA];
 };
 
+// Dynamic shared memory of a candidates CTA: the fixed part, EPC warp scratches, the 256-bit candidate sets per (bin, rotation).
 template <int EPC>
-__global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params P) {
+__host__ __device__ constexpr int cand_smem_bytes(int R) {
+    return (int)((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15) + EPC * WS_BYTES + EPC * R * 8 * 4;
+}
+// Residency the candidates kernel is built for: 32 warps per SM, i.e. 8 CTAs of 4 bins or 4 of 8 -- 1056 / 528 CTA slots on
+// 132 SMs, so a 4096-bin grid (1024 / 512 CTAs) runs in one wave.  The register budget (64 per thread) is enforced through
+// __launch_bounds__, the shared-memory budget below: 228 KB per sm_90 SM, of which the hardware reserves 1 KB per CTA.
+template <int EPC>
+__host__ __device__ constexpr int cand_min_ctas() { return 32 / EPC; }
+constexpr int SM90_SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;
+static_assert(cand_min_ctas<ENVS_PER_CTA_NARROW>() * (cand_smem_bytes<ENVS_PER_CTA_NARROW>(IRBPP_WIDE_MIN_R - 1) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
+              "narrow candidates CTAs at their largest rotation count must fit 32 warps per SM");
+static_assert(cand_min_ctas<ENVS_PER_CTA_WIDE>() * (cand_smem_bytes<ENVS_PER_CTA_WIDE>(IRBPP_WIDE_MIN_R) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
+              "wide candidates CTAs at their smallest rotation count must fit 32 warps per SM");
+
+template <int EPC>
+__global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidates_kernel(const Params P) {
     constexpr int ENVS_PER_CTA = EPC, CAND_WARPS = EPC, CAND_THREADS = 32 * EPC;     // one warp per bin
     extern __shared__ __align__(16) unsigned char smem_raw[];
     CandSmem<EPC>& S = *reinterpret_cast<CandSmem<EPC>*>(smem_raw);
@@ -956,8 +965,8 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
         for (int i = head + 4 * nvec + lane; i < count; i += 32) z0[i] = 0.0f;
     };
 
-    // dynamic tail: CAND_WARPS blocks of P.ws_bytes, then the 256-bit candidate sets per (bin, rotation)
-    uint32_t* candbits = reinterpret_cast<uint32_t*>(smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15) + (size_t)CAND_WARPS * P.ws_bytes);
+    // dynamic tail: CAND_WARPS blocks of WS_BYTES, then the 256-bit candidate sets per (bin, rotation)
+    uint32_t* candbits = reinterpret_cast<uint32_t*>(smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15) + (size_t)CAND_WARPS * WS_BYTES);
     for (int i = tid; i < ENVS_PER_CTA * R * 8; i += CAND_THREADS) candbits[i] = 0u;
     if (tid < ENVS_PER_CTA) S.error[tid] = 0;
     if (warp == 0) {   // prefix of the level counts over the (bin, rotation) pairs, 32 pairs per step
@@ -977,8 +986,8 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
     __syncthreads();
     const int nimg = S.pre[npairs];
     trace(1);
-    unsigned char* ws_base = smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15);     // CAND_WARPS blocks of P.ws_bytes
-    uint8_t* W_pts = ws_base + (size_t)warp * P.ws_bytes;
+    unsigned char* ws_base = smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15);     // CAND_WARPS blocks of WS_BYTES
+    uint8_t* W_pts = ws_base + (size_t)warp * WS_BYTES;
 
     // ---- phase C: rounds of CAND_THREADS level images; inside a round one (image, start pixel) per lane ----
     for (int base = 0; base < nimg; base += CAND_THREADS) {
@@ -1075,19 +1084,14 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
 #endif
 
         // 2. micro-tasks: one (image, start pixel) pair each, TASKS_PER_LANE per lane and batch.  The tasks are in cost
-        //    order, so task slot 0 of the lanes holds the 128 most expensive ones (64-point scratch), slots 1 and 2 the
-        //    cheap rest (32-point scratch): one follow / sort / approximate cycle with its five block barriers serves
-        //    up to 384 tasks -- a 4-bin CTA of the bench workload has ~170
+        //    order, so task slot 0 of the lanes holds the 32 * EPC most expensive ones (FAST_CAP-point scratch), the other
+        //    slots the cheap rest (SLOT_CAP points): one follow / sort / approximate cycle with its five block barriers
+        //    serves up to 32 * EPC * TASKS_PER_LANE tasks -- a 4-bin CTA of the bench workload has ~170
         constexpr int TPL = TASKS_PER_LANE;
         constexpr int BATCH = CAND_THREADS * TPL;
-        static_assert(FAST_CAP * 32 + (TPL - 1) * 32 * 32 <= WS_MIN_BYTES, "the task slots' point buffers share the warp scratch");
-        // points per contour in task slots 1, 2: what the warp scratch holds beside slot 0's 64-point buffers -- 32 at
-        // R <= 4 (4 KB per warp), 64 from R = 8 on (the scratch grows with R for phase D's lists), where long contours
-        // in the cheaper slots are not rare and every overflow is a serial redo
-        const int cap12 = min(FAST_CAP, (P.ws_bytes - FAST_CAP * 32) / ((TPL > 1 ? TPL - 1 : 1) * 32));
         auto slot_scratch = [&](int owner) {               // point buffer of task slot `owner` (j * CAND_THREADS + thread)
             const int jj = owner / CAND_THREADS, th = owner - jj * CAND_THREADS;
-            return ws_base + (size_t)(th >> 5) * P.ws_bytes + (jj == 0 ? 0 : FAST_CAP * 32 + (jj - 1) * cap12 * 32) + (th & 31);
+            return ws_base + (size_t)(th >> 5) * WS_BYTES + (jj == 0 ? 0 : FAST_CAP * 32 + (jj - 1) * SLOT_CAP * 32) + (th & 31);
         };
         for (int mb = 0; mb < ntask; mb += BATCH) {
             int tk[TPL];                                    // slot << 8 | x << 4 | y of my tasks, -1: none
@@ -1121,7 +1125,7 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
                     StridedScratch<32, FAST_CAP> sc;
                     sc.b = slot_scratch(jt * CAND_THREADS + tid);
                     sc.kept = 0;
-                    n = follow_outer_rows(sc, S.slots + slot * ROWS_WORDS, x, y, area2, jt == 0 ? FAST_CAP : cap12);
+                    n = follow_outer_rows(sc, S.slots + slot * ROWS_WORDS, x, y, area2, jt == 0 ? FAST_CAP : SLOT_CAP);
                 }
                 const bool keep = has && n != -2 && area2 <= 0;        // a raster-first start of an outer border
                 if (keep && n < 0) ovf_bits |= 1u << jt;
@@ -1163,7 +1167,7 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
 #ifdef IRBPP_PROBE_FINE
             phase_mark(6);   // length sort
 #endif
-            // (c) lane i approximates the contours of rank i, 128 + i, 256 + i (points live in their owners' scratch)
+            // (c) lane i approximates the contours of rank i, i + CAND_THREADS, ... (points live in their owners' scratch)
 #pragma unroll 1
             for (int jt = 0; jt < TPL; ++jt) {
                 const int owner = S.order2[jt * CAND_THREADS + tid];
@@ -1285,9 +1289,10 @@ __global__ void __launch_bounds__(32 * EPC) irbpp_candidates_kernel(const Params
         // Pass 1 compacts the set bits into a list (no memory loads); pass 2 gives every lane one
         // candidate, so the height gathers of 32 candidates are in flight together.
         // candidate list + bucket-sorted index list: the (now idle) lane scratch, or the pair's slice of the global scratch
-        // (a bin whose candidates fit the warp scratch keeps its lists there even when the global scratch exists)
-        const bool spill = P.dlist && Ktot > P.ws_bytes / 4;
-        const int LIST_CAP = spill ? R * NPOSE : P.ws_bytes / 4;      // >= Ktot
+        // (a bin whose candidates fit the warp scratch keeps its lists there even when the global scratch exists; it is
+        // allocated whenever R * 256 > LIST_CAP_WS)
+        const bool spill = P.dlist && Ktot > LIST_CAP_WS;
+        const int LIST_CAP = spill ? R * NPOSE : LIST_CAP_WS;         // >= Ktot
         uint16_t* list = spill ? P.dlist + (int64_t)env * 2 * (R * NPOSE) : reinterpret_cast<uint16_t*>(W_pts);
         auto cell_of = [](int e) { const int b = e & 255; return (e >> 8) * NPOSE + (b & 15) * 16 + (b >> 4); };
         {

@@ -13,8 +13,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
 import test_kernels_emulated as t  # noqa: E402
+import test_narrow_spill  # noqa: E402
 
 emu = t.build_emulated(tempfile.mkdtemp(), defs=sys.argv[1:] + ["-fsanitize=address", "-g", "-fno-omit-frame-pointer"])
+test_narrow_spill.test_emulated_narrow_shape_list_spill(emu); print("narrow-shape list spill ok")
 t.test_emulated_hull_actions_match_reference_golden(emu); print("hull goldens ok")
 t.test_emulated_survey_known_answers(emu); print("known answers ok")
 t.test_emulated_many_start_pixels(emu); print("many start pixels ok")

@@ -9,7 +9,7 @@
 
 Known build switches (csrc/): IRBPP_PROBE_FINE   slots 4-7 of the phase counters time the sub-phases of phase C
                               IRBPP_PROBE_TRACE  per-CTA timelines of the candidates kernel (tools/cta_trace.py)
-                              IRBPP_TASKS_PER_LANE / IRBPP_ENVS_PER_CTA / IRBPP_ENVS_PER_CTA_WIDE / IRBPP_WIDE_MIN_R / IRBPP_LISTS_SMEM_MAX_R / IRBPP_SCAN_MIN_CTAS   CTA shapes
+                              IRBPP_TASKS_PER_LANE / IRBPP_ENVS_PER_CTA / IRBPP_ENVS_PER_CTA_WIDE / IRBPP_WIDE_MIN_R / IRBPP_SCAN_MIN_CTAS   CTA shapes
 """
 import json
 import os
