@@ -34,6 +34,14 @@ extern "C" {
 #define IRBPP_ESTATE   -3   /* call order violated (e.g. step_async twice; vec_env.py:7-26) */
 #define IRBPP_EDEVICE  -4   /* a kernel flagged an environment error (see irbpp_last_error) */
 
+/* Per-env codes behind IRBPP_EDEVICE (irbpp_step_result.error, "env i reported device error code c"). */
+#define IRBPP_ERR_ACTION    2   /* candidate row / pose out of range */
+#define IRBPP_ERR_ORDER     3   /* get_action_candidates: order action not in [0, k) */
+#define IRBPP_ERR_LEVEL     4   /* a drop height quantised outside the level range */
+#define IRBPP_ERR_TRAJ_END  5   /* the bin drew past the end of its trajectory (irbpp_set_trajectories); the
+                                 * reference appends None there and fails on it (IRcreator.py:94-101) */
+#define IRBPP_ERR_CONTOUR   6   /* a contour longer than the 1024-point overflow buffer */
+
 typedef struct irbpp_env* irbpp_handle;
 
 /* PackingGame.__init__ / Space.__init__ settings that reach the hot path
@@ -58,8 +66,9 @@ typedef struct irbpp_config {
 typedef struct irbpp_step_result {
     const float*   reward;      /* [N]  10*volume/bin_volume on success, 0 otherwise (binPhy.py:299-322) */
     const uint8_t* done;        /* [N]  1 when the placement failed and the bin was auto-reset */
-    const uint8_t* valid;       /* [N]  info['Valid'] (always 1 without the PyBullet settle) */
-    const uint8_t* error;       /* [N]  non-zero: kernel-detected error for that env */
+    const uint8_t* valid;       /* [N]  info['Valid'] (1 without the PyBullet settle; 0 for a bin with no
+                                 *      trajectory left, see irbpp_set_trajectories) */
+    const uint8_t* error;       /* [N]  non-zero: kernel-detected error for that env (IRBPP_ERR_*) */
     const int32_t* counter;     /* [N]  info['counter'] = items packed, meaningful where done */
     const int32_t* ep_len;      /* [N]  info['episode']['l'], meaningful where done */
     const double*  ratio;       /* [N]  info['ratio'] = packed volume / bin volume, where done */
@@ -106,6 +115,30 @@ int irbpp_set_sequences(irbpp_handle h, const int32_t* ids, int32_t length);
  * (splitmix64 finaliser, csrc/irbpp_kernels.cuh item_rng) -- i.i.d. uniform ids without a period, the stand-in
  * for RandomItemCreator (environment/physics0/IRcreator.py:26-33: np.random.choice on every generate_item). */
 int irbpp_set_item_rng(irbpp_handle h, uint64_t seed);
+
+/* Replaces: RandomInstanceCreator / RandomCateCreator (IRcreator.py:35-72; what arguments.py:109-112 selects for
+ * training).  A CSR table of num_groups non-empty groups (host group_offsets int32[G + 1], offsets[0] = 0, strictly
+ * increasing; members int32[offsets[G]] item ids).  Draw d of env e:  z = splitmix64(seed, e, d) (the value
+ * irbpp_set_item_rng keeps the top half of),  g = hi32(z) mod G,  id = members[offsets[g] + lo32(z) mod n_g]:
+ * a group uniformly, then a member uniformly.  The modulo bias is at most G / 2^32 and n_g / 2^32.
+ * Like irbpp_set_sequences it replaces the item source and restarts every bin's item state.
+ * IRBPP_EINVAL on an empty group, offsets that do not increase, or an id out of range. */
+int irbpp_set_item_groups(irbpp_handle h, uint64_t seed, int32_t num_groups, const int32_t* group_offsets,
+                          const int32_t* members);
+
+/* Replaces: LoadItemCreator (IRcreator.py:74-101) over test_sequence.pt, the evaluation protocol of tools.test.
+ * A pool of num_trajectories ragged trajectories (host items int32[offsets[T]], offsets int64[T + 1], offsets[0] = 0,
+ * non-decreasing) and a window [first, first + count).  Episode j of env e (j counts the env's resets and
+ * auto-resets since this call) plays trajectory t = first + e + j * N from its item 0; every draw (the reset's
+ * preview of max(k, 1) items, the refill after each placement) takes the next item.  With N = 1 and first = 1
+ * this is tools.test's sequence of trajectories.  A draw past the end of a trajectory is error code
+ * IRBPP_ERR_TRAJ_END.  When t >= first + count the env is idle: every call leaves its state alone, its
+ * observation rows are zero, its step reports reward 0, done 0, valid 0, error 0 whatever the action, and
+ * irbpp_heuristic_actions returns index -1 for it.  Replaces the item source and restarts every bin's item state.
+ * IRBPP_EINVAL on an id out of range, decreasing offsets, a window outside the pool or a trajectory of the window
+ * shorter than the reset's preview. */
+int irbpp_set_trajectories(irbpp_handle h, const int32_t* items, const int64_t* offsets, int32_t num_trajectories,
+                           int32_t first, int32_t count);
 
 /* Replaces: envs.reset() (envs.py:149-152 -> ShmemVecEnv.reset, shmem_vec_env.py:60-66; and
  * reset_specific, :113-118, when `which` (host uint8[N], 1 = reset) is not NULL).

@@ -36,6 +36,8 @@ SIGNATURES = {
     "irbpp_load_shapes": (c_i32, [c_void_p, c_i32, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_i64]),
     "irbpp_set_sequences": (c_i32, [c_void_p, c_void_p, c_i32]),
     "irbpp_set_item_rng": (c_i32, [c_void_p, ctypes.c_uint64]),
+    "irbpp_set_item_groups": (c_i32, [c_void_p, ctypes.c_uint64, c_i32, c_void_p, c_void_p]),
+    "irbpp_set_trajectories": (c_i32, [c_void_p, c_void_p, c_void_p, c_i32, c_i32, c_i32]),
     "irbpp_reset": (c_i32, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "irbpp_step_async": (c_i32, [c_void_p, c_void_p, c_i32, c_void_p, c_void_p]),
     "irbpp_step_wait": (c_i32, [c_void_p, ctypes.POINTER(IrbppStepResult)]),

@@ -10,6 +10,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <functional>
 #include <mutex>
 #include <cmath>
 #include <string>
@@ -54,6 +55,8 @@ struct irbpp_env {
     // shape pools
     ShapeRot* srot_dev = nullptr; double* Bs_dev = nullptr; double* Ts_dev = nullptr;
     double* vol_dev = nullptr; double* rew_dev = nullptr; int32_t* seq_dev = nullptr;
+    int32_t* grp_off_dev = nullptr; int32_t* grp_mem_dev = nullptr;
+    int32_t* traj_items_dev = nullptr; int64_t* traj_off_dev = nullptr;
     TileEntry* tiles_dev = nullptr;
     unsigned long long* phase_dev = nullptr;
 };
@@ -127,12 +130,20 @@ static cudaError_t raise_dynamic_smem(int device, int which, int bytes) {
     std::lock_guard<std::mutex> lk(mu);
     if (device < 0 || device >= 64) return cudaErrorInvalidDevice;
     if (bytes <= raised[device][which]) return cudaSuccess;
-    cudaError_t e = which == 0
-        ? cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_NARROW>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)
-        : which == 3
-        ? cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)
-        : (which == 1 ? cudaFuncSetAttribute(irbpp_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)
-                      : cudaFuncSetAttribute(irbpp_shape_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    const cudaFuncAttribute a = cudaFuncAttributeMaxDynamicSharedMemorySize;
+    cudaError_t e = cudaSuccess;
+    if (which == 0) {
+        e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, false>, a, bytes);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, true>, a, bytes);
+    } else if (which == 3) {
+        e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, false>, a, bytes);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, true>, a, bytes);
+    } else if (which == 1) {
+        e = cudaFuncSetAttribute(irbpp_scan_kernel<false>, a, bytes);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(irbpp_scan_kernel<true>, a, bytes);
+    } else {
+        e = cudaFuncSetAttribute(irbpp_shape_encode_kernel, a, bytes);
+    }
     if (e == cudaSuccess) raised[device][which] = bytes;
     return e;
 }
@@ -397,15 +408,36 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
     return IRBPP_OK;
 }
 
-// fresh per-bin state: cursors restart, every bin's first sequence entry is staged for its first draw
-static int restart_items(irbpp_env* h, const int32_t* ids, int32_t length) {
+// fresh per-bin state: cursors restart, `init(e, state)` stages what the bin's first draw needs
+static int restart_items(irbpp_env* h, const std::function<void(int, EnvState&)>& init) {
     std::vector<EnvState> st((size_t)h->P.N);
     memset(st.data(), 0, st.size() * sizeof(EnvState));
-    if (ids) for (int e = 0; e < h->P.N; ++e) st[e].next_seq = ids[(size_t)e * length];
+    for (int e = 0; e < h->P.N; ++e) init(e, st[e]);
     CUDA_TRY(h, cudaDeviceSynchronize());
     CUDA_TRY(h, cudaMemcpy(h->P.state, st.data(), st.size() * sizeof(EnvState), cudaMemcpyHostToDevice));
     h->was_reset = false;
     h->scan_current = false;
+    return IRBPP_OK;
+}
+
+// a new item source replaces the previous one and its device pools
+static int drop_item_pools(irbpp_env* h) {
+    CUDA_TRY(h, cudaDeviceSynchronize());
+    for (void* old : {(void*)h->seq_dev, (void*)h->grp_off_dev, (void*)h->grp_mem_dev, (void*)h->traj_items_dev, (void*)h->traj_off_dev})
+        free_dev(h, old);
+    h->seq_dev = nullptr; h->grp_off_dev = nullptr; h->grp_mem_dev = nullptr; h->traj_items_dev = nullptr; h->traj_off_dev = nullptr;
+    Params& P = h->P;
+    P.seq = nullptr; P.L = 0; P.grp_off = nullptr; P.grp_mem = nullptr; P.G = 0;
+    P.traj_items = nullptr; P.traj_off = nullptr; P.traj_end = 0;
+    h->sequences_set = false;
+    return IRBPP_OK;
+}
+
+static int upload(irbpp_env* h, void** dst, const void* src, size_t bytes) {
+    char* p = nullptr;
+    CUDA_TRY(h, dev_alloc(h, &p, bytes, false));
+    *dst = p;
+    if (bytes) CUDA_TRY(h, cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice));
     return IRBPP_OK;
 }
 
@@ -416,12 +448,10 @@ int irbpp_set_sequences(irbpp_handle h, const int32_t* ids, int32_t length) {
     for (size_t i = 0; i < n; ++i)
         if (ids[i] < 0 || ids[i] >= h->P.S) return fail(h, IRBPP_EINVAL, "item id %d out of range at %zu", ids[i], i);
     DeviceGuard guard(h->cfg.device);
-    CUDA_TRY(h, cudaDeviceSynchronize());
-    free_dev(h, h->seq_dev); h->seq_dev = nullptr;                       // a reload replaces the previous pool
-    CUDA_TRY(h, dev_alloc(h, &h->seq_dev, n, false));
-    CUDA_TRY(h, cudaMemcpy(h->seq_dev, ids, n * 4, cudaMemcpyHostToDevice));
-    int rc = restart_items(h, ids, length); if (rc) return rc;
-    h->P.seq = h->seq_dev; h->P.L = length;
+    int rc = drop_item_pools(h); if (rc) return rc;
+    rc = upload(h, (void**)&h->seq_dev, ids, n * 4); if (rc) return rc;
+    rc = restart_items(h, [&](int e, EnvState& s) { s.next_seq = ids[(size_t)e * length]; }); if (rc) return rc;
+    h->P.item_src = ITEMS_SEQ; h->P.seq = h->seq_dev; h->P.L = length;
     h->sequences_set = true;
     return IRBPP_OK;
 }
@@ -430,8 +460,68 @@ int irbpp_set_item_rng(irbpp_handle h, uint64_t seed) {
     if (!h) return IRBPP_EINVAL;
     if (!h->shapes_loaded) return fail(h, IRBPP_ESTATE, "load shapes before the item generator");
     DeviceGuard guard(h->cfg.device);
-    int rc = restart_items(h, nullptr, 0); if (rc) return rc;
-    h->P.seq = nullptr; h->P.L = 0; h->P.rng_seed = seed;
+    int rc = drop_item_pools(h); if (rc) return rc;
+    rc = restart_items(h, [](int, EnvState&) {}); if (rc) return rc;
+    h->P.item_src = ITEMS_RNG; h->P.rng_seed = seed;
+    h->sequences_set = true;
+    return IRBPP_OK;
+}
+
+int irbpp_set_item_groups(irbpp_handle h, uint64_t seed, int32_t num_groups, const int32_t* group_offsets,
+                          const int32_t* members) {
+    if (!h) return IRBPP_EINVAL;
+    if (!group_offsets || !members || num_groups <= 0) return fail(h, IRBPP_EINVAL, "bad item groups");
+    if (!h->shapes_loaded) return fail(h, IRBPP_ESTATE, "load shapes before the item groups");
+    if (group_offsets[0] != 0) return fail(h, IRBPP_EINVAL, "group_offsets[0] must be 0");
+    for (int g = 0; g < num_groups; ++g)
+        if (group_offsets[g + 1] <= group_offsets[g])
+            return fail(h, IRBPP_EINVAL, "group %d is empty or its offsets are not increasing", g);
+    const int32_t M = group_offsets[num_groups];
+    for (int32_t i = 0; i < M; ++i)
+        if (members[i] < 0 || members[i] >= h->P.S) return fail(h, IRBPP_EINVAL, "item id %d out of range at %d", members[i], i);
+    DeviceGuard guard(h->cfg.device);
+    int rc = drop_item_pools(h); if (rc) return rc;
+    if ((rc = upload(h, (void**)&h->grp_off_dev, group_offsets, ((size_t)num_groups + 1) * 4))) return rc;
+    if ((rc = upload(h, (void**)&h->grp_mem_dev, members, (size_t)M * 4))) return rc;
+    rc = restart_items(h, [&](int e, EnvState& s) {     // draw 0 of every bin, staged as sequence mode stages its first entry
+        s.next_seq = group_item(group_offsets, members, num_groups, seed, (uint32_t)e, 0u);
+    });
+    if (rc) return rc;
+    Params& P = h->P;
+    P.item_src = ITEMS_GROUPS; P.rng_seed = seed; P.G = num_groups; P.grp_off = h->grp_off_dev; P.grp_mem = h->grp_mem_dev;
+    h->sequences_set = true;
+    return IRBPP_OK;
+}
+
+int irbpp_set_trajectories(irbpp_handle h, const int32_t* items, const int64_t* offsets, int32_t num_trajectories,
+                           int32_t first, int32_t count) {
+    if (!h) return IRBPP_EINVAL;
+    if (!items || !offsets || num_trajectories <= 0) return fail(h, IRBPP_EINVAL, "bad trajectories");
+    if (!h->shapes_loaded) return fail(h, IRBPP_ESTATE, "load shapes before the trajectories");
+    if (first < 0 || count < 0 || (int64_t)first + count > num_trajectories)
+        return fail(h, IRBPP_EINVAL, "window [%d, %d + %d) outside the %d trajectories", first, first, count, num_trajectories);
+    if (offsets[0] != 0) return fail(h, IRBPP_EINVAL, "offsets[0] must be 0");
+    for (int t = 0; t < num_trajectories; ++t)
+        if (offsets[t + 1] < offsets[t]) return fail(h, IRBPP_EINVAL, "offsets decrease at trajectory %d", t);
+    const int64_t M = offsets[num_trajectories];
+    for (int64_t i = 0; i < M; ++i)
+        if (items[i] < 0 || items[i] >= h->P.S) return fail(h, IRBPP_EINVAL, "item id %d out of range at %lld", items[i], (long long)i);
+    const int nfill = h->P.K > 1 ? h->P.K : 1;       // what reset() previews
+    for (int t = first; t < first + count; ++t)
+        if (offsets[t + 1] - offsets[t] < nfill)
+            return fail(h, IRBPP_EINVAL, "trajectory %d has %lld items, a reset takes %d", t, (long long)(offsets[t + 1] - offsets[t]), nfill);
+    DeviceGuard guard(h->cfg.device);
+    int rc = drop_item_pools(h); if (rc) return rc;
+    if ((rc = upload(h, (void**)&h->traj_items_dev, items, (size_t)M * 4))) return rc;
+    if ((rc = upload(h, (void**)&h->traj_off_dev, offsets, ((size_t)num_trajectories + 1) * 8))) return rc;
+    const int32_t end = first + count;
+    rc = restart_items(h, [&](int e, EnvState& s) {     // episode 0 of bin e plays trajectory first + e
+        const int64_t t = (int64_t)first + e;
+        s.traj_next = (int32_t)(t < end ? t : end);
+    });
+    if (rc) return rc;
+    Params& P = h->P;
+    P.item_src = ITEMS_TRAJ; P.traj_items = h->traj_items_dev; P.traj_off = h->traj_off_dev; P.traj_end = end;
     h->sequences_set = true;
     return IRBPP_OK;
 }
@@ -458,7 +548,10 @@ static int launch(irbpp_env* h, Params& P, cudaStream_t s) {
     if (++h->epoch == 0) h->epoch = 1;
     P.epoch = h->epoch;
     if (P.mode == MODE_DEBUG_HULLS) irbpp_levels_kernel<<<P.N, CTA_THREADS, 0, s>>>(P);
-    else irbpp_scan_kernel<<<units, CTA_THREADS, h->scan_smem, s>>>(P);
+    else {
+        void (*scan)(const Params) = P.item_src == ITEMS_TRAJ ? irbpp_scan_kernel<true> : irbpp_scan_kernel<false>;
+        scan<<<units, CTA_THREADS, h->scan_smem, s>>>(P);
+    }
     h->launches += 1;
     if (mode_emits_loc(P.mode, P.K)) {
         // programmatic dependent launch: the candidates grid is scheduled while the scan grid's last
@@ -470,8 +563,11 @@ static int launch(irbpp_env* h, Params& P, cudaStream_t s) {
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = (P.mode == MODE_DEBUG_HULLS) ? 0 : 1;
         lc.attrs = at; lc.numAttrs = 1;
-        if (h->epc == ENVS_PER_CTA_WIDE) cudaLaunchKernelEx(&lc, irbpp_candidates_kernel<ENVS_PER_CTA_WIDE>, P);
-        else cudaLaunchKernelEx(&lc, irbpp_candidates_kernel<ENVS_PER_CTA_NARROW>, P);
+        const bool traj = P.item_src == ITEMS_TRAJ;
+        void (*cand)(const Params) = h->epc == ENVS_PER_CTA_WIDE
+            ? (traj ? irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, true> : irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, false>)
+            : (traj ? irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, true> : irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, false>);
+        cudaLaunchKernelEx(&lc, cand, P);
         h->launches += 1;
     }
     cudaError_t e = cudaGetLastError();

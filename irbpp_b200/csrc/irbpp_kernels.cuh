@@ -122,11 +122,24 @@ struct EnvState {
     double vol_sum;            // packed volume (get_ratio, binPhy.py:149-153)
     double ep_rew;             // sum of episode rewards (monitor.py:60)
     int32_t queue[MAX_QUEUE];  // item FIFO (IRcreator.py:6-24)
-    int32_t next_seq;          // the sequence entry the next draw returns (fetched one draw ahead: off the step's critical path)
-    int32_t seq_pos;           // cursor modulo the sequence length, kept incrementally
-    int32_t pad[4];
+    int32_t next_seq;          // the id the next draw returns (fetched one draw ahead: off the step's critical path)
+    int32_t seq_pos;           // sequences: cursor modulo the sequence length; trajectories: index of next_seq in the trajectory
+    // trajectory replay (ITEMS_TRAJ) only
+    int64_t traj_base;         // first item of the current trajectory in the pool
+    int32_t traj_next;         // trajectory the bin's next reset starts (first + e + j N)
+    int32_t traj_len;          // items of the current trajectory; TRAJ_IDLE: no trajectory left for this bin
 };
 static_assert(sizeof(EnvState) == 128, "EnvState must be 128 bytes");
+constexpr int32_t TRAJ_IDLE = -1;
+constexpr int ERR_TRAJ_END = 5;        // a draw past the end of the bin's trajectory (IRBPP_EDEVICE code 5, include/irbpp.h)
+
+// Where the item ids come from (the reference's item creators, IRcreator.py)
+enum ItemSource : int {
+    ITEMS_RNG = 0,         // counter-based uniform ids (RandomItemCreator)
+    ITEMS_SEQ = 1,         // per-bin sequences replayed modulo their length
+    ITEMS_GROUPS = 2,      // a group uniformly, then an id uniformly within it (RandomInstanceCreator / RandomCateCreator)
+    ITEMS_TRAJ = 3,        // one trajectory per episode from a pool (LoadItemCreator)
+};
 
 struct Params {
     // configuration
@@ -143,9 +156,16 @@ struct Params {
     const double* vol;                   // [S]
     const double* reward_tab;            // [S] (vol / binvol) * 10
     const TileEntry* tiles;              // block form of the bottom tables (tile > 1 entries only)
-    // sequences
-    const int32_t* seq; int32_t L;       // L == 0: ids drawn from the counter-based generator below instead
-    uint64_t rng_seed;
+    // item source (ItemSource)
+    int32_t item_src;
+    const int32_t* seq; int32_t L;       // ITEMS_SEQ
+    uint64_t rng_seed;                   // ITEMS_RNG, ITEMS_GROUPS
+    const int32_t* grp_off;              // ITEMS_GROUPS: CSR table of G non-empty groups, [G + 1]
+    const int32_t* grp_mem;              //   [grp_off[G]] member ids
+    int32_t G;
+    const int32_t* traj_items;           // ITEMS_TRAJ: the pool's ids
+    const int64_t* traj_off;             //   [T + 1] start of every trajectory
+    int32_t traj_end;                    //   first + count: trajectories from here on are not played
     // per-env state
     double* hm;                          // [N][2][32][16] column-parity planes
     uint16_t* cand;                      // [N][cand_stride] rot<<8 | x<<4 | y  (rows padded to 16 bytes: bulk-copied)
@@ -182,33 +202,75 @@ struct Params {
 
 __device__ __forceinline__ int hm_index(int x, int y) { return ((y & 1) * HX + x) * (HY / 2) + (y >> 1); }
 
-// Counter-based item generator (stand-in for RandomItemCreator, IRcreator.py:26-33, when no explicit sequences
-// are loaded): id = mix(seed, env, draw counter) mod S -- i.i.d. uniform ids, no period, no memory.
-__host__ __device__ __forceinline__ uint32_t item_rng(uint64_t seed, uint32_t env, uint32_t counter) {
-    uint64_t z = seed + 0x9E3779B97F4A7C15ull * (((uint64_t)env << 32) | counter) + 0x9E3779B97F4A7C15ull;   // splitmix64
+// splitmix64 of (seed, env, draw counter): the 64-bit value behind the counter-based item sources
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint32_t env, uint32_t counter) {
+    uint64_t z = seed + 0x9E3779B97F4A7C15ull * (((uint64_t)env << 32) | counter) + 0x9E3779B97F4A7C15ull;
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    return (uint32_t)(z >> 32);
+    return z ^ (z >> 31);
 }
 
-// generate_item (IRcreator.py:17-24): the id at the bin's cursor.  With explicit sequences the entry was fetched
-// by the previous draw (EnvState::next_seq) and this draw fetches the one after it.
+// Counter-based item generator (stand-in for RandomItemCreator, IRcreator.py:26-33): id = mix(seed, env, draw
+// counter) mod S -- i.i.d. uniform ids, no period, no memory.
+__host__ __device__ __forceinline__ uint32_t item_rng(uint64_t seed, uint32_t env, uint32_t counter) {
+    return (uint32_t)(splitmix64(seed, env, counter) >> 32);
+}
+
+// Grouped draw (RandomInstanceCreator / RandomCateCreator, IRcreator.py:35-72): group g = hi32(z) mod G, then
+// member lo32(z) mod n_g of it.  Both modulos are biased by at most G / 2^32 and n_g / 2^32.
+__host__ __device__ __forceinline__ int group_item(const int32_t* off, const int32_t* mem, int G, uint64_t seed,
+                                                   uint32_t env, uint32_t counter) {
+    const uint64_t z = splitmix64(seed, env, counter);
+    const uint32_t g = (uint32_t)(z >> 32) % (uint32_t)G;
+    const int32_t o = off[g];
+    return mem[o + (int32_t)((uint32_t)z % (uint32_t)(off[g + 1] - o))];
+}
+
+// generate_item (IRcreator.py:17-24).  Except for the uniform generator the id was fetched by the previous draw
+// (EnvState::next_seq) and this draw fetches the one after it.
 // `next` is the caller's register copy of EnvState::next_seq: the load issued here is consumed by the NEXT draw
 // (normally in the next step; the caller stores it back with the state), so nothing waits for it.
-__device__ __forceinline__ int draw_item(const Params& P, int env, EnvState& st, int& next) {
-    if (P.L == 0) {
+// A trajectory that has no item left sets `err` (the reference appends None and fails on it) and returns id 0.
+template <bool TRAJ>
+__device__ __forceinline__ int draw_item(const Params& P, int env, EnvState& st, int& next, int& err) {
+    if (P.item_src == ITEMS_RNG) {
         const int id = (int)(item_rng(P.rng_seed, (uint32_t)env, (uint32_t)st.cursor) % (uint32_t)P.S);
         st.cursor += 1;
         return id;
     }
-    const int id = next;
-    int pos = st.seq_pos + 1;
-    if (pos >= P.L) pos = 0;
-    st.seq_pos = pos;
+    int id = next;
     st.cursor += 1;
-    next = P.seq[(int64_t)env * P.L + pos];
+    if (!TRAJ && P.item_src == ITEMS_SEQ) {
+        int pos = st.seq_pos + 1;
+        if (pos >= P.L) pos = 0;
+        st.seq_pos = pos;
+        next = P.seq[(int64_t)env * P.L + pos];
+    } else if (!TRAJ) {
+        next = group_item(P.grp_off, P.grp_mem, P.G, P.rng_seed, (uint32_t)env, (uint32_t)st.cursor);
+    } else {
+        if (st.seq_pos >= st.traj_len) { err = ERR_TRAJ_END; id = 0; }
+        const int pos = st.seq_pos + 1;
+        st.seq_pos = pos;
+        next = pos < st.traj_len ? P.traj_items[st.traj_base + pos] : 0;
+    }
     return id;
+}
+
+// reset() of LoadItemCreator (IRcreator.py:82-92): the bin's next trajectory, from item 0.  `b`, `e` are
+// traj_off[traj_next] and traj_off[traj_next + 1], loaded by the caller ahead of time.  Returns false when the
+// bin has no trajectory left (it turns idle).
+__device__ __forceinline__ bool begin_trajectory(const Params& P, EnvState& st, int& next, int64_t b, int64_t e) {
+    if (st.traj_next >= P.traj_end) { st.traj_len = TRAJ_IDLE; return false; }
+    st.traj_base = b;
+    st.traj_len = (int32_t)(e - b);
+    st.seq_pos = 0;
+    const int64_t t = (int64_t)st.traj_next + P.N;
+    st.traj_next = (int32_t)(t < P.traj_end ? t : P.traj_end);
+    next = st.traj_len > 0 ? P.traj_items[b] : 0;
+    return true;
+}
+__device__ __forceinline__ bool env_idle(const Params& P, int env) {
+    return P.item_src == ITEMS_TRAJ && P.state[env].traj_len == TRAJ_IDLE;
 }
 
 __host__ __device__ __forceinline__ bool mode_emits_loc(int mode, int K) {
@@ -443,6 +505,8 @@ constexpr int READY_POLLS = 1 << 16;       // ~10 ms of polling before the fallb
 #ifndef IRBPP_SCAN_MIN_CTAS
 #define IRBPP_SCAN_MIN_CTAS 8
 #endif
+// TRAJ: the item source is trajectory replay (idle bins exist); the other sources run the instantiation without that code
+template <bool TRAJ>
 __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_kernel(const Params P) {
     __shared__ __align__(128) double hm_s[HX * HY];
     extern __shared__ __align__(16) TileEntry estage[];  // CTA_WARPS x P.maxwh: scan list of each warp's rotation
@@ -450,7 +514,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     __shared__ double M_s[NPOSE];                        // block maxima of the heightmap (block form of phase B)
     __shared__ double P2_s[NPOSE];                       // 2x2 block maxima
     __shared__ double z_sh;
-    __shared__ int ok_sh, rot_sh, lx_sh, ly_sh, item_sh, err_sh, any_sh;
+    __shared__ int ok_sh, rot_sh, lx_sh, ly_sh, item_sh, err_sh, any_sh;   // item_sh < 0: the bin is idle (no trajectory left)
     __shared__ __align__(8) mbarrier_t mbar;             // completion of the bulk copies of this bin's inputs
     __shared__ __align__(16) ShapeRot srot_s[MAX_ROT];   // (56 bytes each) table headers of the item the action places (all rotations), prefetched
     __shared__ long long a_sh;                           // the bin's action
@@ -508,7 +572,14 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     }
     if (tid == 0) { err_sh = 0; any_sh = 0; }
     __syncthreads();                       // mbarrier initialised, state in shared memory
-    if (mode == MODE_STEP) {
+    // trajectory replay: a bin with no trajectory left ignores every call (no draw, no placement, no error)
+    const bool idle_in = TRAJ && st_s.traj_len == TRAJ_IDLE && mode != MODE_DEBUG_SCAN;
+    int64_t tb_pf = 0, te_pf = 0;          // thread 0: bounds of the trajectory a reset / auto-reset would start
+    if (TRAJ && tid == 0 && !idle_in && (mode == MODE_STEP || mode == MODE_RESET) &&
+        st_s.traj_next < P.traj_end) {
+        tb_pf = P.traj_off[st_s.traj_next]; te_pf = P.traj_off[st_s.traj_next + 1];
+    }
+    if (mode == MODE_STEP && !idle_in) {
         // while the bulk copies land: the table headers of the item to be placed, all rotations (48 bytes each), so
         // that decoding the action does not start another round trip to L2
         static_assert(sizeof(ShapeRot) % 8 == 0, "headers are copied as 8-byte words");
@@ -522,7 +593,10 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
 
     int32_t* queue_g = st_s.queue;
     int next_seq = st_s.next_seq;          // thread 0's register copy; written back with the state
-    auto draw = [&]() { return draw_item(P, env, st_s, next_seq); };
+    int draw_err = 0;                      // thread 0: ERR_TRAJ_END of a draw past the trajectory's end
+    auto draw = [&]() { return draw_item<TRAJ>(P, env, st_s, next_seq, draw_err); };
+    // thread 0, reset / auto-reset: the next trajectory; false when the bin turns idle
+    auto new_episode = [&]() { return !TRAJ || begin_trajectory(P, st_s, next_seq, tb_pf, te_pf); };
     // zero the bin's heightmap in global memory (reset / auto-reset); the shared copy is zeroed by the caller
     auto zero_hm_global = [&]() {
         double2* dst = reinterpret_cast<double2*>(hm_g);
@@ -531,13 +605,29 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     bool st_dirty = false;
 
     // ---- phase A: bookkeeping / apply action ----
-    if (mode == MODE_RESET) {
+    if (idle_in) {
+        if (tid == 0) {
+            item_sh = -1;
+            if (mode == MODE_STEP) {       // reward 0, done 0, Valid 0: trainer-style loops skip the bin
+                P.r_reward[env] = 0.0f; P.r_done[env] = 0; P.r_valid[env] = 0;
+                P.r_counter[env] = -1; P.r_eplen[env] = 0; P.r_ratio[env] = -1.0; P.r_eprew[env] = 0.0;
+                if (P.h_reward) {
+                    P.h_reward[env] = 0.0f; P.h_done[env] = 0; P.h_valid[env] = 0;
+                    P.h_counter[env] = -1; P.h_eplen[env] = 0; P.h_ratio[env] = -1.0; P.h_eprew[env] = 0.0;
+                }
+            }
+        }
+        __syncthreads();
+    } else if (mode == MODE_RESET) {
         if (tid == 0) {
             const int nfill = P.K > 1 ? P.K : 1;
-            for (int q = 0; q < nfill; ++q) queue_g[q] = draw();
+            const bool live = new_episode();
+            if (live)
+                for (int q = 0; q < nfill; ++q) queue_g[q] = draw();
+            if (draw_err) err_sh = draw_err;
             st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0;
             st_s.order_act = 0;
-            item_sh = queue_g[0];
+            item_sh = live ? queue_g[0] : -1;
         }
         zero_hm_global();
         st_dirty = true;
@@ -609,6 +699,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         }
         if (tid == 0) {
             const int nfill = P.K > 1 ? P.K : 1;
+            bool live = true;
             if (ok) {
                 const double rew = rew_pf;
                 P.r_reward[env] = (float)rew; P.r_done[env] = 0; P.r_valid[env] = 1;
@@ -637,9 +728,12 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
                 }
                 st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0;
                 st_s.order_act = 0;
-                for (int q = 0; q < nfill; ++q) queue_g[q] = draw();   // reset(): clear + preview
+                live = new_episode();
+                if (live)
+                    for (int q = 0; q < nfill; ++q) queue_g[q] = draw();   // reset(): clear + preview
             }
-            item_sh = queue_g[0];
+            if (draw_err) err_sh = draw_err;
+            item_sh = live ? queue_g[0] : -1;
         }
         st_dirty = true;
         __syncthreads();
@@ -665,6 +759,23 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     float* obs_g = P.obs + (int64_t)env * P.obs_stride + slot * P.loc_len;
     const int item = item_sh;
     const int ncand = P.sel * 5;
+
+    if (TRAJ && item < 0) {
+        // no trajectory left: an all-zero observation row (no valid candidate); the candidates kernel skips the bin
+        const int width = emit_loc ? P.loc_len : P.order_len;
+        for (int i = tid; i < width; i += CTA_THREADS) obs_g[i] = 0.0f;
+        if (tid == 0) {
+            if (mode != MODE_ALL_OBS) { P.r_error[env] = (uint8_t)err_sh; if (P.h_error) P.h_error[env] = (uint8_t)err_sh; }
+            st_s.next_seq = next_seq;
+        }
+        __syncthreads();
+        if (st_dirty && warp == 0) reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st_s)[lane];
+        if (P.ready) {
+            __syncthreads();
+            if (tid == 0) ready_publish(P.ready + vb, P.epoch);
+        }
+        return;
+    }
 
     // the heightmap is final for this call: float32 copy into the observation, state write-back
     {
@@ -793,6 +904,13 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
     __shared__ int idx_sh;
     const int env = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (env_idle(P, env)) {               // no trajectory left: no pose
+        if (tid == 0) {
+            P.heur_pose[env * 3 + 0] = 0; P.heur_pose[env * 3 + 1] = 0; P.heur_pose[env * 3 + 2] = 0;
+            P.heur_index[env] = -1;
+        }
+        return;
+    }
     const int item = P.state[env].cur_item;
     const int method = P.heur_method;
     if (method == HEUR_HM) {
@@ -900,7 +1018,7 @@ static_assert(cand_min_ctas<ENVS_PER_CTA_NARROW>() * (cand_smem_bytes<ENVS_PER_C
 static_assert(cand_min_ctas<ENVS_PER_CTA_WIDE>() * (cand_smem_bytes<ENVS_PER_CTA_WIDE>(IRBPP_WIDE_MIN_R) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
               "wide candidates CTAs at their smallest rotation count must fit 32 warps per SM");
 
-template <int EPC>
+template <int EPC, bool TRAJ>      // TRAJ: as in irbpp_scan_kernel
 __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidates_kernel(const Params P) {
     constexpr int ENVS_PER_CTA = EPC, CAND_WARPS = EPC, CAND_THREADS = 32 * EPC;     // one warp per bin
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -944,11 +1062,14 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
 #else
     auto trace = [&](int, unsigned long long = 0ull) {};
 #endif
-    auto env_live = [&](int e) { return !(P.mode == MODE_RESET && P.which && !P.which[e]); };
     // the "bins" of this kernel are (bin, buffer slot) pairs in MODE_ALL_OBS (see the scan kernel): real bin, slot and
     // the place of a pair's rows in the observation
     const bool all_obs = (P.mode == MODE_ALL_OBS);
     auto real_env = [&](int e) { return all_obs ? e / P.K : e; };
+    // bins not reset by a partial reset, and idle bins (their scan CTA wrote the zero observation row), have no phase C / D
+    auto env_live = [&](int e) {
+        return !(P.mode == MODE_RESET && P.which && !P.which[e]) && !(TRAJ && P.mode != MODE_DEBUG_HULLS && env_idle(P, real_env(e)));
+    };
     auto slot_of_e = [&](int e) { return all_obs ? e % P.K : 0; };
     auto obs_offset = [&](int e) { return (int64_t)real_env(e) * P.obs_stride + slot_of_e(e) * P.loc_len; };
     // Zero the candidate rows [first, sel) of one bin's observation (one warp): scalar stores up to a 16-byte

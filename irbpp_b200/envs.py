@@ -10,9 +10,11 @@ path reads (``binPhy.py:25-49``):
 
 plus the shape data: ``args.shapeLibrary`` (a ``shapes.ShapeLibrary``) or the reference's own
 ``args.shotInfo`` / ``args.shapeDict`` (extents) / ``args.infoDict`` (volumes), and optionally
-``args.itemSequences`` (int ids ``[num_processes, L]``, replayed modulo L).  Without it the ids are drawn
-i.i.d. uniform ON THE DEVICE from a counter-based generator seeded with ``args.seed`` -- the role of
-``RandomItemCreator`` (``IRcreator.py:26-33``); there is no period.  ``args.approxLegacy`` (optional, default
+``args.itemSequences`` (int ids ``[num_processes, L]``, replayed modulo L).  Without it the ids are drawn ON THE
+DEVICE, seeded with ``args.seed``, as the reference's ``args.dataSample`` selects (``binPhy.py:58-67``): 'instance' /
+'category' draw a group uniformly, then an id within it, from the groups of the id -> file dict ``args.dicPath``
+(``RandomInstanceCreator`` / ``RandomCateCreator``, ``IRcreator.py:35-72``); 'pose' or no ``dataSample`` draws
+i.i.d. uniform ids (``RandomItemCreator``, ``IRcreator.py:26-33``).  Neither has a period.  ``args.approxLegacy`` (optional, default
 False) selects the older point-to-line ``approxPolyDP`` rule (the reference pins OpenCV 4.4.0.46)."""
 import numpy as np
 
@@ -42,13 +44,48 @@ def make_vec_envs(args, log_dir=None, allow_early_resets=True):
     if lib is None:
         lib = library_from_reference_args(args)
     n = int(args.num_processes)
-    seqs = getattr(args, "itemSequences", None)        # None: i.i.d. ids generated on the device
-    envs = GpuVecEnv(lib, seqs, num_envs=n, device=getattr(args, "device", "cuda:0"),
-                     item_seed=int(getattr(args, "seed", 0)), approx_legacy=bool(getattr(args, "approxLegacy", False)),
-                     selected_action=int(getattr(args, "selectedAction", 500)),
-                     buffer_size=int(getattr(args, "bufferSize", 1)),
-                     bin_dimension=tuple(getattr(args, "bin_dimension", (0.32, 0.32, 0.30))),
-                     resolution_act=float(getattr(args, "resolutionA", 0.02)),
-                     resolution_h=float(getattr(args, "resolutionH", 0.01)),
-                     resolution_z=float(getattr(args, "resolutionZ", 0.01)))
+    seqs = getattr(args, "itemSequences", None)
+    groups = None
+    if seqs is None:
+        groups = item_groups_from_args(args)           # None: i.i.d. uniform ids generated on the device
+    envs = GpuVecEnv(lib, seqs, num_envs=n, device=getattr(args, "device", "cuda:0"), item_groups=groups,
+                     item_seed=int(getattr(args, "seed", 0)), **_env_kwargs(args))
     return envs, [envs.observation_space, envs.action_space], envs.obs_len
+
+
+def _env_kwargs(args):
+    return dict(approx_legacy=bool(getattr(args, "approxLegacy", False)),
+                selected_action=int(getattr(args, "selectedAction", 500)),
+                buffer_size=int(getattr(args, "bufferSize", 1)),
+                bin_dimension=tuple(getattr(args, "bin_dimension", (0.32, 0.32, 0.30))),
+                resolution_act=float(getattr(args, "resolutionA", 0.02)),
+                resolution_h=float(getattr(args, "resolutionH", 0.01)),
+                resolution_z=float(getattr(args, "resolutionZ", 0.01)))
+
+
+def item_groups_from_args(args):
+    """The groups ``binPhy.py:58-67`` builds its item creator from: ``args.dataSample`` 'instance' ->
+    ``shapes.instance_groups``, 'category' -> ``shapes.category_groups`` of the id -> file dict ``args.dicPath`` (a
+    path loaded with ``torch.load``, or the dict itself); 'pose' or no ``dataSample``: None (uniform ids)."""
+    sample = getattr(args, "dataSample", None)
+    if sample in (None, "pose"):
+        return None
+    if sample not in ("instance", "category"):
+        raise ValueError("unknown dataSample %r" % (sample,))
+    d = args.dicPath
+    if not isinstance(d, dict):
+        import torch
+        d = torch.load(d, weights_only=False)
+    return shapes.instance_groups(d) if sample == "instance" else shapes.category_groups(d)
+
+
+def make_eval_env(args):
+    """``make_eval_env`` (reference ``tools.py:433``): one bin that plays the trajectories of ``args.test_name`` (a
+    ``test_sequence.pt`` path, or the list itself) from trajectory 1 on, as ``LoadItemCreator`` does under
+    ``tools.test``."""
+    from .single_env import SingleGpuEnv
+    lib = getattr(args, "shapeLibrary", None)
+    if lib is None:
+        lib = library_from_reference_args(args)
+    return SingleGpuEnv(lib, trajectories=shapes.load_trajectories(args.test_name), first_trajectory=1,
+                        device=getattr(args, "device", "cuda:0"), **_env_kwargs(args))

@@ -372,6 +372,12 @@ def item_rng_ids(seed, num_envs, count, num_shapes):
     ``mix(seed, e, d) mod num_shapes`` with the splitmix64 finaliser of ``csrc/irbpp_kernels.cuh``
     (``item_rng``).  Returns ``ids[num_envs, count]`` int32 -- used by the tests to give the CPU oracle
     the very same i.i.d. stream (the stand-in for ``RandomItemCreator``, reference ``IRcreator.py:26-33``)."""
+    z = _splitmix64(seed, num_envs, count)
+    return ((z >> np.uint64(32)) % np.uint64(num_shapes)).astype(np.int32)
+
+
+def _splitmix64(seed, num_envs, count):
+    """``splitmix64(seed, e, d)`` of ``csrc/irbpp_kernels.cuh`` for every env e and draw d: uint64 [num_envs, count]."""
     M = np.uint64(0xFFFFFFFFFFFFFFFF)
     e = np.arange(num_envs, dtype=np.uint64)[:, None]
     d = np.arange(count, dtype=np.uint64)[None, :]
@@ -380,5 +386,73 @@ def item_rng_ids(seed, num_envs, count, num_shapes):
         z = (np.uint64(seed) + g * ((e << np.uint64(32)) | d) + g) & M
         z = ((z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)) & M
         z = ((z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)) & M
-        z = z ^ (z >> np.uint64(31))
-    return ((z >> np.uint64(32)) % np.uint64(num_shapes)).astype(np.int32)
+        return z ^ (z >> np.uint64(31))
+
+
+def instance_groups(id2shape):
+    """The groups ``RandomInstanceCreator`` draws from (reference ``IRcreator.py:35-50``): the ids of the id -> file
+    dict (``args.dicPath``) keyed by ``name[0:-6]`` -- the file name without its pose suffix -- in the order the dict
+    lists them.  Returns a list of id lists."""
+    inverse = {}
+    for k, name in id2shape.items():
+        inverse.setdefault(name[0:-6], []).append(k)
+    return list(inverse.values())
+
+
+CATEGORIES = ("objects", "concave", "board")     # IRcreator.py:55; the declared weights are never used
+
+
+def category_groups(id2shape):
+    """The groups ``RandomCateCreator`` draws from (reference ``IRcreator.py:52-72``): the ids of each of the fixed
+    categories ``objects / concave / board``, by the ``category/file`` prefix of their name; the category is chosen
+    uniformly.  An empty category raises ``ValueError`` (the reference would fail at its first draw)."""
+    cates = {c: [] for c in CATEGORIES}
+    for k, name in id2shape.items():
+        cate, _ = name.split("/")
+        if cate not in cates:
+            raise ValueError("unknown category %r of item %r" % (cate, k))
+        cates[cate].append(k)
+    for c, ids in cates.items():
+        if not ids:
+            raise ValueError("category %r has no item" % c)
+    return list(cates.values())
+
+
+def group_table(groups):
+    """Groups (lists of ids) -> the CSR form of ``irbpp_set_item_groups``: ``(offsets int32[G + 1], members int32)``."""
+    sizes = [len(g) for g in groups]
+    offsets = np.zeros(len(groups) + 1, dtype=np.int32)
+    offsets[1:] = np.cumsum(sizes)
+    members = np.array([int(i) for g in groups for i in g], dtype=np.int32)
+    return offsets, members
+
+
+def item_group_ids(seed, num_envs, count, groups):
+    """The ids the device draws with item groups (``irbpp_set_item_groups``): env e's d-th draw takes
+    ``z = splitmix64(seed, e, d)``, group ``hi32(z) mod G`` and member ``lo32(z) mod n_g`` of it.  Returns
+    ``ids[num_envs, count]`` int32 -- the Python mirror of the device stream."""
+    offsets, members = group_table(groups)
+    z = _splitmix64(seed, num_envs, count)
+    g = ((z >> np.uint64(32)) % np.uint64(len(groups))).astype(np.int64)
+    lo = z & np.uint64(0xFFFFFFFF)
+    n = (offsets[g + 1] - offsets[g]).astype(np.uint64)
+    return members[offsets[g] + (lo % n).astype(np.int64)].astype(np.int32)
+
+
+def load_trajectories(path_or_list):
+    """Item trajectories as ``LoadItemCreator`` reads them (reference ``IRcreator.py:74-80``): ``test_sequence.pt`` is
+    a ``torch.load``-ed list of id lists.  Accepts that path or the list itself; returns a list of int lists (a copy:
+    the reference's creator appends ``None`` to the lists it plays)."""
+    trajs = path_or_list
+    if isinstance(path_or_list, (str, bytes)) or hasattr(path_or_list, "__fspath__"):
+        import torch
+        trajs = torch.load(path_or_list, weights_only=False)
+    return [[int(i) for i in t] for t in trajs]
+
+
+def trajectory_table(trajectories):
+    """Trajectories -> the ragged form of ``irbpp_set_trajectories``: ``(items int32, offsets int64[T + 1])``."""
+    offsets = np.zeros(len(trajectories) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([len(t) for t in trajectories])
+    items = np.array([int(i) for t in trajectories for i in t], dtype=np.int32)
+    return items, offsets

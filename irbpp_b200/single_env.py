@@ -18,13 +18,21 @@ from .vec_env import GpuVecEnv
 
 class _ItemCreatorView(object):
     def __init__(self):
-        self.traj_index = 0          # episodes started so far (LoadItemCreator.traj_index, IRcreator.py:78-92)
+        # LoadItemCreator.traj_index (IRcreator.py:78-92): with trajectories, the one the current episode plays
+        # (first_trajectory, first_trajectory + 1, ...); otherwise the number of episodes started so far
+        self.traj_index = 0
 
 
 class SingleGpuEnv(object):
-    def __init__(self, library, sequence=None, **kw):
+    """``trajectories`` (a list of id lists, ``shapes.load_trajectories``) replays them as ``LoadItemCreator`` does:
+    every ``reset()`` moves to the next one, starting at ``first_trajectory`` (1, as ``tools.test`` plays them)."""
+
+    def __init__(self, library, sequence=None, trajectories=None, first_trajectory=1, **kw):
         seqs = None if sequence is None else np.asarray(sequence, dtype=np.int32).reshape(1, -1)
+        if trajectories is not None:
+            kw.update(trajectories=trajectories, first_trajectory=first_trajectory)
         self._venv = GpuVecEnv(library, seqs, num_envs=1, **kw)
+        self._replay = trajectories is not None
         self.library = library
         self.obs_len = self._venv.obs_len
         self.observation_space, self.action_space = self._venv.observation_space, self._venv.action_space
@@ -40,7 +48,10 @@ class SingleGpuEnv(object):
         else:
             obs = self._venv.reset().cpu().numpy()[0]
         self.packed = []
-        self.item_creator.traj_index += 1
+        if self._replay:
+            self.item_creator.traj_index = int(self._venv.trajectory[0])
+        else:
+            self.item_creator.traj_index += 1
         if self._venv.buffer_size == 1:
             self._last = obs
         return obs

@@ -22,7 +22,7 @@ from collections.abc import Sequence
 
 import numpy as np
 
-from . import _lib
+from . import _lib, shapes
 
 
 class AlreadySteppingError(Exception):
@@ -180,17 +180,32 @@ class GpuVecEnv(VecEnv):
     ``sequences`` the per-env item ids ``[N, L]`` (replayed modulo L; what the parity tests use), or ``None``
     for i.i.d. ids generated on the device from ``item_seed`` (the stand-in for ``RandomItemCreator``,
     IRcreator.py:26-33).  ``approx_legacy`` selects the point-to-line ``approxPolyDP`` rule believed to be
-    what the reference's pinned OpenCV 4.4.0.46 computes (default: the 4.13 rule, the one testable here)."""
+    what the reference's pinned OpenCV 4.4.0.46 computes (default: the 4.13 rule, the one testable here).
+
+    Two more item sources, each exclusive with ``sequences``:
+
+    * ``item_groups``: a list of id lists (``shapes.instance_groups`` / ``shapes.category_groups``); every draw picks
+      a group uniformly, then an id uniformly within it, on the device, seeded with ``item_seed``
+      (``RandomInstanceCreator`` / ``RandomCateCreator``, IRcreator.py:35-72).
+    * ``trajectories``: a list of id lists (``shapes.load_trajectories``), played as ``LoadItemCreator`` plays them
+      (IRcreator.py:74-101): episode j of bin e plays trajectory ``first_trajectory + e + j * N`` from its first item,
+      over the window of ``num_trajectories`` (default: all from ``first_trajectory`` on).  ``trajectory[e]`` is the
+      trajectory bin e plays (-1 before its first reset); a bin whose next trajectory lies beyond the window is
+      ``idle``: zero observation rows, reward 0, done False, ``info['Valid']`` False, its actions ignored.  Both are
+      followed on the host from resets and the ``done`` flags ``step_wait`` returns."""
 
     def __init__(self, library, sequences, num_envs=None, device="cuda:0", selected_action=500, buffer_size=1,
                  bin_dimension=(0.32, 0.32, 0.30), resolution_act=0.02, resolution_h=0.01, resolution_z=0.01,
-                 approx_legacy=False, item_seed=0):
+                 approx_legacy=False, item_seed=0, item_groups=None, trajectories=None, first_trajectory=1,
+                 num_trajectories=None):
         import torch
         self._torch = torch
         self._lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("GpuVecEnv needs a CUDA device; there is no CPU path")
+        if sum(x is not None for x in (sequences, item_groups, trajectories)) > 1:
+            raise ValueError("sequences, item_groups and trajectories are mutually exclusive")
         if sequences is None:
             # no explicit sequences: ids are drawn on the device, i.i.d. uniform from a counter-based generator
             # seeded with ``item_seed`` (RandomItemCreator's role, IRcreator.py:26-33; no period)
@@ -227,10 +242,26 @@ class GpuVecEnv(VecEnv):
                                          dims.ctypes.data, ext.ctypes.data, vol.ctypes.data, maps.ctypes.data,
                                          offsets.ctypes.data, maps.size)
         self._check(rc)
-        if sequences is None:
-            rc = self._lib.irbpp_set_item_rng(self._h, int(item_seed) & 0xFFFFFFFFFFFFFFFF)
-        else:
+        seed = int(item_seed) & 0xFFFFFFFFFFFFFFFF
+        self._traj_window = None
+        if sequences is not None:
             rc = self._lib.irbpp_set_sequences(self._h, sequences.ctypes.data, sequences.shape[1])
+        elif item_groups is not None:
+            goff, gmem = shapes.group_table(item_groups)
+            self._keep += (goff, gmem)
+            rc = self._lib.irbpp_set_item_groups(self._h, seed, len(item_groups), goff.ctypes.data, gmem.ctypes.data)
+        elif trajectories is not None:
+            items, toff = shapes.trajectory_table(trajectories)
+            first = int(first_trajectory)
+            count = len(trajectories) - first if num_trajectories is None else int(num_trajectories)
+            rc = self._lib.irbpp_set_trajectories(self._h, items.ctypes.data, toff.ctypes.data, len(trajectories),
+                                                  first, count)
+            self._traj_window = (first, first + count)
+            self._traj_next = first + np.arange(num_envs, dtype=np.int64)     # what each bin's next reset starts
+            self.trajectory = np.full(num_envs, -1, dtype=np.int64)
+            self.idle = np.zeros(num_envs, dtype=np.bool_)
+        else:
+            rc = self._lib.irbpp_set_item_rng(self._h, seed)
         self._check(rc)
         o, l, k = _lib.c_i32(), _lib.c_i32(), _lib.c_i32()
         self._check(self._lib.irbpp_obs_len(self._h, ctypes.byref(o), ctypes.byref(l), ctypes.byref(k)))
@@ -287,6 +318,7 @@ class GpuVecEnv(VecEnv):
         obs = self._new_obs(self.obs_len)
         self._check(self._lib.irbpp_reset(self._h, None, obs.data_ptr(), self._stream()))
         self._tstart = time.time()
+        self._new_episodes(slice(None))
         return obs
 
     def reset_specific(self, indexs, obs):
@@ -296,7 +328,19 @@ class GpuVecEnv(VecEnv):
         which[np.asarray(indexs, dtype=np.int64)] = 1
         self._check(self._lib.irbpp_reset(self._h, which.ctypes.data, obs.data_ptr(), self._stream()))
         self._torch.cuda.current_stream(self.device).synchronize()   # `which` is read asynchronously
+        self._new_episodes(which.astype(np.bool_))
         return obs
+
+    def _new_episodes(self, bins):
+        """Trajectory replay: the listed bins were reset (or auto-reset) -- each starts its next trajectory, or turns
+        idle when that one lies beyond the window (the device applies the same rule, include/irbpp.h)."""
+        if self._traj_window is None:
+            return
+        t = self._traj_next[bins]
+        live = t < self._traj_window[1]
+        self.idle[bins] = ~live
+        self.trajectory[bins] = np.where(live, t, -1)
+        self._traj_next[bins] = np.where(live, t + self.num_envs, t)
 
     def _take_obs(self):
         """Observation buffer of the step being launched: the one ``step_wait`` allocated while the GPU
@@ -339,6 +383,7 @@ class GpuVecEnv(VecEnv):
         reward = src[offs["reward"]:offs["reward"] + 4 * n].view(np.float32).copy()
         done = src[offs["done"]:offs["done"] + n].view(np.bool_).copy()
         infos = LazyInfos(n, src, offs, done, t_rel, borrowed=True)
+        self._new_episodes(done)
         self._live_infos = (self._live_infos + [weakref.ref(infos)])[-2:]
         return obs, torch.from_numpy(reward).unsqueeze(dim=1), done, infos
 
@@ -376,6 +421,8 @@ class GpuVecEnv(VecEnv):
         keep, ptr, on_dev = self._actions_arg(actions, "actions")
         if not on_dev:
             raise ValueError("step_device needs a CUDA tensor")
+        if self._traj_window is not None:
+            raise ValueError("trajectory replay follows episodes through the done flags of step / step_wait")
         obs = self._new_obs(self.obs_len)
         self._check(self._lib.irbpp_step_async(self._h, ptr, 1, obs.data_ptr(), self._stream()))
         res = self._result

@@ -14,9 +14,15 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
 import test_kernels_emulated as t  # noqa: E402
 import test_narrow_spill  # noqa: E402
+import test_item_sources  # noqa: E402
 
 emu = t.build_emulated(tempfile.mkdtemp(), defs=sys.argv[1:] + ["-fsanitize=address", "-g", "-fno-omit-frame-pointer"])
 test_narrow_spill.test_emulated_narrow_shape_list_spill(emu); print("narrow-shape list spill ok")
+for k in (1, 5):
+    test_item_sources.test_emulated_trajectories_match_oracle_until_idle(emu, k); print("trajectories k=%d ok" % k)
+test_item_sources.test_emulated_grouped_stream_matches_mirror(emu); print("grouped draws ok")
+test_item_sources.test_emulated_trajectory_end_is_error_5(emu); print("trajectory end ok")
+test_item_sources.test_emulated_bad_tables_are_rejected(emu); print("bad tables ok")
 t.test_emulated_hull_actions_match_reference_golden(emu); print("hull goldens ok")
 t.test_emulated_survey_known_answers(emu); print("known answers ok")
 t.test_emulated_many_start_pixels(emu); print("many start pixels ok")
