@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define IRBPP_ABI_VERSION 1
+#define IRBPP_ABI_VERSION 2
 
 #define IRBPP_OK        0
 #define IRBPP_EINVAL   -1   /* bad argument / unsupported configuration */
@@ -252,6 +252,78 @@ int irbpp_shape_features(const float* shape_array, int32_t S, int32_t P, const f
                          int32_t item_col, const int32_t* ids, int32_t B, uint64_t seed, uint64_t counter,
                          int32_t n_points, const float* W1, const float* b1, const float* W2, const float* b2,
                          float negative_slope, int32_t* scratch_keys, float* out, void* stream);
+
+/* ---- prioritized n-step replay (memory.py:15-208) -------------------------------------------------------------
+ * Replaces: the N host ReplayMemory objects of main.py:61-63, their per-bin appends (trainer.py:184-186), the per-memory
+ * sample of Agent.learn (agent.py:69-82) and its per-transition priority write-back (agent.py:123-124).  M memories of
+ * capacity C share caller-owned DEVICE arrays, memory-major; handle-free; errors through irbpp_last_error(NULL).
+ *   states float32 [M][C][obs_len], timesteps int32 [M][C], actions int64 [M][C], rewards float32 [M][C],
+ *   nonterminals uint8 [M][C], tree float32 [M][2C-1] (heap layout: leaf j is node C-1+j), state [M] below.
+ * The reference stores actions as float32 and returns them as int64, which is exact below 2^24; they are kept as
+ * int64 here.  Every call issues one kernel on `stream`. */
+typedef struct irbpp_replay_state {
+    int32_t index;             /* next ring slot to write */
+    int32_t full;              /* the ring has wrapped at least once */
+    int32_t t;                 /* timestep within the current episode */
+    float   max;               /* running maximum priority, starts at 1, never decreases */
+} irbpp_replay_state;
+
+typedef struct irbpp_replay_memory {
+    int32_t num_memories, capacity, obs_len;   /* M, C >= 2, obs_len */
+    float* states;
+    int32_t* timesteps;
+    int64_t* actions;
+    float* rewards;
+    uint8_t* nonterminals;
+    float* tree;
+    irbpp_replay_state* state;
+} irbpp_replay_memory;
+
+/* Outputs of one sample call, device arrays of B = G * k rows (row g * k + i is stratum i of memory mem_ids[g]):
+ * tree_idx int64 [B] (-1 where the sample failed), states / next_states float32 [B][obs_len], actions int64 [B],
+ * returns / nonterminals / weights float32 [B]; attempts int32 [B] (descents used) and error int32 [B]
+ * (IRBPP_REPLAY_ERR_*) may be NULL. */
+typedef struct irbpp_replay_batch {
+    int64_t* tree_idx;
+    float* states;
+    int64_t* actions;
+    float* returns;
+    float* next_states;
+    float* nonterminals;
+    float* weights;
+    int32_t* attempts;
+    int32_t* error;
+} irbpp_replay_batch;
+
+/* Per-sample codes; a device error word (uint32, may be NULL) gets bit (1 << code) for every code reported. */
+#define IRBPP_REPLAY_ERR_STARVED  1   /* no valid leaf in `max_attempts` descents of the stratum (the reference loops
+                                       * forever there: memory.py:163-170) */
+#define IRBPP_REPLAY_ERR_MEMORY   2   /* sample: memory id out of range */
+#define IRBPP_REPLAY_ERR_INDEX    3   /* update: memory id or tree index out of range; the row is ignored */
+
+/* Empty memories: tree zero, state {0, 0, 0, 1.0f} (memory.py:23-34).  The ring arrays need no initialisation. */
+int irbpp_replay_init(const irbpp_replay_memory* mem, void* stream);
+
+/* ReplayMemory.append (memory.py:110-113) for every memory m with valid[m] != 0 (valid may be NULL: all):
+ * (t, obs[m * obs_stride ...], action[m], reward[m], !done[m]) at slot index with priority max, then index, full and t
+ * advance.  obs float32, action int64, reward float32, done / valid uint8, all device, [M] rows.  reward_clip > 0 clamps
+ * the reward to [-reward_clip, reward_clip] first (trainer.py:181-182). */
+int irbpp_replay_append(const irbpp_replay_memory* mem, const float* obs, int64_t obs_stride, const int64_t* action,
+                        const float* reward, const uint8_t* done, const uint8_t* valid, float reward_clip, void* stream);
+
+/* ReplayMemory.sample(k) (memory.py:191-203) for each of the G memories of mem_ids (device int32 [G]), n = multi_step
+ * (0 <= n < C, n <= 64), discount gamma, importance exponent beta.  Stratum i draws lo + (hi - lo) * U with
+ * U = uniforms[row * max_attempts + a] (device float64, may be NULL) or, when uniforms is NULL, a counter-based
+ * splitmix64 uniform of (seed, call, row, a) with 53 bits; at most max_attempts (1..65536) descents per stratum. */
+int irbpp_replay_sample(const irbpp_replay_memory* mem, const int32_t* mem_ids, int32_t G, int32_t k, int32_t n,
+                        double discount, double beta, int32_t max_attempts, uint64_t seed, uint64_t call,
+                        const double* uniforms, const irbpp_replay_batch* out, uint32_t* error_flags, void* stream);
+
+/* ReplayMemory.update_priorities for a whole batch (agent.py:123-124, memory.py:206-208): row r sets leaf tree_idxs[r]
+ * of memory mem_ids[r] to float32 loss[r] ** omega; rows of one memory apply in batch order (a duplicated index keeps
+ * the last value), each with its ancestors, and max rises to the largest value set.  Device int32 / int64 / float32 [B]. */
+int irbpp_replay_update_priorities(const irbpp_replay_memory* mem, const int32_t* mem_ids, const int64_t* tree_idxs,
+                                   const float* loss, int32_t B, double omega, uint32_t* error_flags, void* stream);
 
 /* Profiling aid: when enabled, thread 0 of every CTA adds the SM cycles it spent in each kernel phase
  * (0 scan kernel: load + apply action, 1 scan kernel: observation heightmap + scan + level bitmaps,

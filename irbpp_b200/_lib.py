@@ -12,7 +12,7 @@ c_i32, c_i64, c_f64 = ctypes.c_int32, ctypes.c_int64, ctypes.c_double
 c_void_p, c_char_p = ctypes.c_void_p, ctypes.c_char_p
 
 IRBPP_OK, IRBPP_EINVAL, IRBPP_ECUDA, IRBPP_ESTATE, IRBPP_EDEVICE = 0, -1, -2, -3, -4
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 class IrbppConfig(ctypes.Structure):
@@ -24,6 +24,17 @@ class IrbppConfig(ctypes.Structure):
 class IrbppStepResult(ctypes.Structure):
     _fields_ = [("reward", c_void_p), ("done", c_void_p), ("valid", c_void_p), ("error", c_void_p),
                 ("counter", c_void_p), ("ep_len", c_void_p), ("ratio", c_void_p), ("ep_reward", c_void_p)]
+
+
+class IrbppReplayMemory(ctypes.Structure):
+    _fields_ = [("num_memories", c_i32), ("capacity", c_i32), ("obs_len", c_i32), ("states", c_void_p),
+                ("timesteps", c_void_p), ("actions", c_void_p), ("rewards", c_void_p), ("nonterminals", c_void_p),
+                ("tree", c_void_p), ("state", c_void_p)]
+
+
+class IrbppReplayBatch(ctypes.Structure):
+    _fields_ = [(n, c_void_p) for n in ("tree_idx", "states", "actions", "returns", "next_states", "nonterminals",
+                                         "weights", "attempts", "error")]
 
 
 # symbol -> (restype, argtypes); every symbol of include/irbpp.h appears here (checked by the tests)
@@ -61,6 +72,14 @@ SIGNATURES = {
                                      ctypes.c_uint64, c_i32, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_float,
                                      c_void_p, c_void_p, c_void_p]),
     "irbpp_debug_phase_cycles": (c_i32, [c_void_p, c_i32, c_void_p]),
+    "irbpp_replay_init": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p]),
+    "irbpp_replay_append": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, ctypes.c_float, c_void_p]),
+    "irbpp_replay_sample": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_i32, c_i32, c_i32, c_f64, c_f64, c_i32,
+                                    ctypes.c_uint64, ctypes.c_uint64, c_void_p, ctypes.POINTER(IrbppReplayBatch),
+                                    c_void_p, c_void_p]),
+    "irbpp_replay_update_priorities": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_void_p, c_void_p, c_i32,
+                                               c_f64, c_void_p, c_void_p]),
 }
 
 _LIB = None

@@ -20,6 +20,7 @@
 #include "irbpp_kernels.cuh"
 #include "irbpp_pointnet.cuh"
 #include "irbpp_pack.cuh"
+#include "irbpp_replay.cuh"
 
 using namespace irbpp;
 
@@ -957,6 +958,83 @@ int irbpp_shape_features(const float* shape_array, int32_t S, int32_t P, const f
     e = cudaGetLastError();
     if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "kernel launch: %s", cudaGetErrorString(e));
     return IRBPP_OK;
+}
+
+// ---- prioritized n-step replay (csrc/irbpp_replay.cuh) ---------------------------------------------------------
+static int replay_check(const irbpp_replay_memory* mem) {
+    if (!mem) return fail(nullptr, IRBPP_EINVAL, "null replay memory");
+    if (mem->num_memories <= 0 || mem->capacity < 2 || mem->obs_len <= 0)
+        return fail(nullptr, IRBPP_EINVAL, "bad replay sizes (M %d, C %d, obs_len %d; need M > 0, C >= 2, obs_len > 0)",
+                    mem->num_memories, mem->capacity, mem->obs_len);
+    if ((int64_t)mem->capacity * 2 - 1 > INT32_MAX) return fail(nullptr, IRBPP_EINVAL, "replay capacity too large");
+    if (!mem->states || !mem->timesteps || !mem->actions || !mem->rewards || !mem->nonterminals || !mem->tree || !mem->state)
+        return fail(nullptr, IRBPP_EINVAL, "null replay array");
+    return IRBPP_OK;
+}
+
+static int launch_status() {
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "kernel launch: %s", cudaGetErrorString(e));
+    return IRBPP_OK;
+}
+
+int irbpp_replay_init(const irbpp_replay_memory* mem, void* stream) {
+    int rc = replay_check(mem); if (rc) return rc;
+    const int dev = device_of(mem->tree);
+    DeviceGuard guard(dev);
+    const int64_t nodes = (int64_t)mem->num_memories * (2 * mem->capacity - 1);
+    const int blocks = (int)std::min<int64_t>((nodes + 255) / 256, gather_grid_cap(dev));
+    irbpp_replay_init_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(*mem);
+    return launch_status();
+}
+
+int irbpp_replay_append(const irbpp_replay_memory* mem, const float* obs, int64_t obs_stride, const int64_t* action,
+                        const float* reward, const uint8_t* done, const uint8_t* valid, float reward_clip, void* stream) {
+    int rc = replay_check(mem); if (rc) return rc;
+    if (!obs || !action || !reward || !done) return fail(nullptr, IRBPP_EINVAL, "null append input");
+    if (obs_stride < mem->obs_len) return fail(nullptr, IRBPP_EINVAL, "observation stride %lld < obs_len %d", (long long)obs_stride, mem->obs_len);
+    ReplayAppendArgs A;
+    A.mem = *mem; A.obs = obs; A.obs_stride = obs_stride; A.action = action; A.reward = reward; A.done = done; A.valid = valid;
+    A.reward_clip = reward_clip;
+    DeviceGuard guard(device_of(mem->tree));
+    irbpp_replay_append_kernel<<<mem->num_memories, RP_APPEND_THREADS, 0, (cudaStream_t)stream>>>(A);
+    return launch_status();
+}
+
+int irbpp_replay_sample(const irbpp_replay_memory* mem, const int32_t* mem_ids, int32_t G, int32_t k, int32_t n,
+                        double discount, double beta, int32_t max_attempts, uint64_t seed, uint64_t call,
+                        const double* uniforms, const irbpp_replay_batch* out, uint32_t* error_flags, void* stream) {
+    int rc = replay_check(mem); if (rc) return rc;
+    if (!mem_ids || !out) return fail(nullptr, IRBPP_EINVAL, "null sample argument");
+    if (G < 1 || k < 1) return fail(nullptr, IRBPP_EINVAL, "need G >= 1 memories and k >= 1 samples each (G %d, k %d)", G, k);
+    if ((int64_t)G * k > INT32_MAX) return fail(nullptr, IRBPP_EINVAL, "batch too large");
+    if (n < 0 || n >= mem->capacity || n > RP_MAX_N)
+        return fail(nullptr, IRBPP_EINVAL, "multi_step %d outside [0, min(C - 1, %d)] (C %d)", n, RP_MAX_N, mem->capacity);
+    if (max_attempts < 1 || max_attempts > 65536) return fail(nullptr, IRBPP_EINVAL, "max_attempts %d outside [1, 65536]", max_attempts);
+    if (!out->tree_idx || !out->states || !out->actions || !out->returns || !out->next_states || !out->nonterminals || !out->weights)
+        return fail(nullptr, IRBPP_EINVAL, "null sample output");
+    ReplaySampleArgs A;
+    memset(&A, 0, sizeof(A));
+    A.mem = *mem; A.mem_ids = mem_ids; A.G = G; A.k = k; A.n = n; A.attempts = max_attempts;
+    for (int i = 0; i < n; ++i) A.scale[i] = (float)std::pow(discount, (double)i);     // torch.tensor([γ ** i], float32)
+    A.neg_beta = (double)(float)(-beta);
+    A.seed = seed; A.call = call; A.uniforms = uniforms; A.out = *out; A.error_flags = error_flags;
+    DeviceGuard guard(device_of(mem->tree));
+    irbpp_replay_sample_kernel<<<G, RP_SAMPLE_THREADS, 0, (cudaStream_t)stream>>>(A);
+    return launch_status();
+}
+
+int irbpp_replay_update_priorities(const irbpp_replay_memory* mem, const int32_t* mem_ids, const int64_t* tree_idxs,
+                                   const float* loss, int32_t B, double omega, uint32_t* error_flags, void* stream) {
+    int rc = replay_check(mem); if (rc) return rc;
+    if (B < 1 || !mem_ids || !tree_idxs || !loss) return fail(nullptr, IRBPP_EINVAL, "bad update arguments (B %d)", B);
+    ReplayUpdateArgs A;
+    A.mem = *mem; A.mem_ids = mem_ids; A.tree_idxs = tree_idxs; A.loss = loss; A.B = B;
+    A.omega = (double)(float)omega; A.error_flags = error_flags;
+    DeviceGuard guard(device_of(mem->tree));
+    const int blocks = (mem->num_memories + RP_UPDATE_WARPS - 1) / RP_UPDATE_WARPS;
+    irbpp_replay_update_kernel<<<blocks, 32 * RP_UPDATE_WARPS, 0, (cudaStream_t)stream>>>(A);
+    return launch_status();
 }
 
 int irbpp_debug_phase_cycles(irbpp_handle h, int32_t enable, uint64_t* out8) {

@@ -28,6 +28,16 @@ class StandInAgent(object):
         return q.argmax(1)
 
 
+def count_kernels(fn):
+    """Kernels (not copies or memsets) that one call of fn puts on the GPU, from torch.profiler's CUDA events."""
+    from torch.profiler import profile, ProfilerActivity
+    fn(); torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn(); torch.cuda.synchronize()
+    return sum(1 for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+               and "memcpy" not in e.name.lower() and "memset" not in e.name.lower())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=30)
@@ -90,6 +100,42 @@ def main():
     out["glue_loop"] = {"iters_per_s": a.iters / dt, "env_steps_per_s": n * a.iters / dt, "episodes": stats.episodes,
                         "mean_ratio_last10": float(np.mean(stats.episode_ratio)) if stats.episode_ratio else None,
                         "ms_per_iter_by_part": {k: round(1e3 * v / a.iters, 4) for k, v in parts.items()}}
+
+    # ---- the prioritized bank (memory.py's replay, csrc/irbpp_replay.cuh) beside the uniform bank ----
+    pbank = glue.PrioritizedReplayBank(n, a.capacity, env.obs_len, dev, seed=1)
+    ubank = glue.ReplayBank(n, a.capacity, env.obs_len, dev)
+    pparts = {"prioritized append": 0.0, "prioritized sample": 0.0, "prioritized update": 0.0,
+              "uniform append": 0.0, "uniform sample": 0.0}
+    parts = pparts
+    rounds = 0
+    for T in range(1, a.iters + 1):
+        action = agent.act(state, glue.get_mask_from_state(state, SEL))
+        next_state, reward, done, infos = env.step(action.cpu().numpy())
+        torch.cuda.synchronize(); t = time.perf_counter()
+        ubank.append_from_env(env, state, action, reward_clip=10.0)
+        t = lap("uniform append", t)
+        pbank.append_from_env(env, state, action, reward_clip=10.0)
+        t = lap("prioritized append", t)
+        if T >= a.capacity // 2:
+            ubank.sample(a.batch_size)
+            t = lap("uniform sample", t)
+            batch = pbank.sample(a.batch_size)
+            t = lap("prioritized sample", t)
+            loss = torch.rand(batch[0].shape[0], device=dev)
+            torch.cuda.synchronize(); t = time.perf_counter()
+            pbank.update_priorities(batch[0], batch[7], loss)
+            t = lap("prioritized update", t)
+            rounds += 1
+        state = next_state
+    out["replay_banks"] = {"ms_per_call": {k: round(1e3 * v / (a.iters if "append" in k else max(rounds, 1)), 4)
+                                           for k, v in pparts.items()},
+                           "kernel_launches_per_call": {
+                               "prioritized append": count_kernels(lambda: pbank.append_from_env(env, state, action)),
+                               "prioritized sample": count_kernels(lambda: pbank.sample(a.batch_size)),
+                               "prioritized update": count_kernels(lambda: pbank.update_priorities(batch[0], batch[7], loss)),
+                               "uniform append": count_kernels(lambda: ubank.append_from_env(env, state, action)),
+                               "uniform sample": count_kernels(lambda: ubank.sample(a.batch_size))},
+                           "sample_rounds": rounds, "capacity": a.capacity, "batch_size": a.batch_size}
 
     # ---- the loop as trainer.py:157-186 writes it (per-bin Python) ----
     if not a.skip_reference_style:
