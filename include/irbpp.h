@@ -75,17 +75,8 @@ typedef struct irbpp_step_result {
     const double*  ep_reward;   /* [N]  unrounded sum of episode rewards (Monitor rounds to 6 dp) */
 } irbpp_step_result;
 
-/* Device-resident copies of the same arrays (for callers that keep the loop on the GPU). */
-typedef struct irbpp_device_result {
-    const float*   reward;
-    const uint8_t* done;
-    const uint8_t* valid;
-    const uint8_t* error;
-    const int32_t* counter;
-    const int32_t* ep_len;
-    const double*  ratio;
-    const double*  ep_reward;
-} irbpp_device_result;
+/* The same struct pointing at the device-resident copies of the arrays (for callers that keep the loop on the GPU). */
+typedef irbpp_step_result irbpp_device_result;
 
 int irbpp_abi_version(void);
 

@@ -5,6 +5,8 @@ device is present ``irbpp_create`` fails with ``IRBPP_ECUDA``."""
 import ctypes
 import os
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("IRBPP_LIB") or os.path.join(HERE, "lib", "libirbpp.so")   # IRBPP_LIB: build-variant experiments
 
@@ -24,6 +26,12 @@ class IrbppConfig(ctypes.Structure):
 class IrbppStepResult(ctypes.Structure):
     _fields_ = [("reward", c_void_p), ("done", c_void_p), ("valid", c_void_p), ("error", c_void_p),
                 ("counter", c_void_p), ("ep_len", c_void_p), ("ratio", c_void_p), ("ep_reward", c_void_p)]
+
+
+# The arrays irbpp_step_result points at, in the order of the library's result block, with their element types
+RESULT_FIELDS = tuple((name, np.dtype(t)) for name, t in (
+    ("ratio", np.float64), ("ep_reward", np.float64), ("reward", np.float32), ("counter", np.int32), ("ep_len", np.int32),
+    ("done", np.uint8), ("valid", np.uint8), ("error", np.uint8)))
 
 
 class IrbppReplayMemory(ctypes.Structure):

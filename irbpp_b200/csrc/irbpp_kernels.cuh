@@ -141,6 +141,19 @@ enum ItemSource : int {
     ITEMS_TRAJ = 3,        // one trajectory per episode from a pool (LoadItemCreator)
 };
 
+// The per-bin results of a step, one array each, in the order of the result block (8-byte fields first, so every
+// array stays aligned).  irbpp.cu's step_results() is the only place that cuts a block into these arrays.
+struct StepResults {
+    double* ratio;
+    double* ep_reward;
+    float* reward;
+    int32_t* counter;
+    int32_t* ep_len;
+    uint8_t* done;
+    uint8_t* valid;
+    uint8_t* error;
+};
+
 struct Params {
     // configuration
     int32_t N, R, sel, K;                // K = buffer_size (1 = online)
@@ -190,17 +203,32 @@ struct Params {
     int32_t env_lo, env_hi;              // bins [env_lo, env_hi) handled by this launch (the full range [0, N))
     // outputs
     float* obs;                          // [N][obs_stride] (+ slot offset in MODE_ALL_OBS)
-    float* r_reward; uint8_t* r_done; uint8_t* r_valid; uint8_t* r_error;
-    int32_t* r_counter; int32_t* r_eplen; double* r_ratio; double* r_eprew;
+    StepResults res;                     // the device result block
     double* dbg_cand; int32_t* dbg_nhull;
-    // host-mapped mirror of the result arrays (zero-copy stores; NULL on the device-resident path)
-    float* h_reward; uint8_t* h_done; uint8_t* h_valid; uint8_t* h_error;
-    int32_t* h_counter; int32_t* h_eplen; double* h_ratio; double* h_eprew;
+    StepResults res_host;                // host-mapped block of a step with host actions (zero-copy stores), else all NULL
     unsigned long long* phase_cycles;    // [8] summed SM cycles per phase (thread 0 of every CTA), or NULL
     int32_t mode;
 };
 
-__device__ __forceinline__ int hm_index(int x, int y) { return ((y & 1) * HX + x) * (HY / 2) + (y >> 1); }
+// one bin's row of step results, stored to the device block and, when it is set, to the host-mapped block
+__device__ __forceinline__ void store_results(const Params& P, int env, float reward, uint8_t done, uint8_t valid,
+                                              int32_t counter, int32_t ep_len, double ratio, double ep_reward) {
+    auto row = [&](const StepResults& r) {
+        r.reward[env] = reward; r.done[env] = done; r.valid[env] = valid;
+        r.counter[env] = counter; r.ep_len[env] = ep_len; r.ratio[env] = ratio; r.ep_reward[env] = ep_reward;
+    };
+    row(P.res);
+    if (P.res_host.reward) row(P.res_host);
+}
+
+// one bin's error code, stored the same way
+__device__ __forceinline__ void store_error(const Params& P, int env, int err) {
+    P.res.error[env] = (uint8_t)err;
+    if (P.res_host.error) P.res_host.error[env] = (uint8_t)err;
+}
+
+// cell (x, y) of a bin's heightmap in the column-parity planes: [y & 1][x][y >> 1]
+__host__ __device__ __forceinline__ int hm_index(int x, int y) { return ((y & 1) * HX + x) * (HY / 2) + (y >> 1); }
 
 // splitmix64 of (seed, env, draw counter): the 64-bit value behind the counter-based item sources
 __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint32_t env, uint32_t counter) {
@@ -608,14 +636,8 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     if (idle_in) {
         if (tid == 0) {
             item_sh = -1;
-            if (mode == MODE_STEP) {       // reward 0, done 0, Valid 0: trainer-style loops skip the bin
-                P.r_reward[env] = 0.0f; P.r_done[env] = 0; P.r_valid[env] = 0;
-                P.r_counter[env] = -1; P.r_eplen[env] = 0; P.r_ratio[env] = -1.0; P.r_eprew[env] = 0.0;
-                if (P.h_reward) {
-                    P.h_reward[env] = 0.0f; P.h_done[env] = 0; P.h_valid[env] = 0;
-                    P.h_counter[env] = -1; P.h_eplen[env] = 0; P.h_ratio[env] = -1.0; P.h_eprew[env] = 0.0;
-                }
-            }
+            if (mode == MODE_STEP)         // reward 0, done 0, Valid 0: trainer-style loops skip the bin
+                store_results(P, env, 0.0f, 0, 0, -1, 0, -1.0, 0.0);
         }
         __syncthreads();
     } else if (mode == MODE_RESET) {
@@ -702,12 +724,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
             bool live = true;
             if (ok) {
                 const double rew = rew_pf;
-                P.r_reward[env] = (float)rew; P.r_done[env] = 0; P.r_valid[env] = 1;
-                P.r_counter[env] = -1; P.r_eplen[env] = 0; P.r_ratio[env] = -1.0; P.r_eprew[env] = 0.0;
-                if (P.h_reward) {
-                    P.h_reward[env] = (float)rew; P.h_done[env] = 0; P.h_valid[env] = 1;
-                    P.h_counter[env] = -1; P.h_eplen[env] = 0; P.h_ratio[env] = -1.0; P.h_eprew[env] = 0.0;
-                }
+                store_results(P, env, (float)rew, 0, 1, -1, 0, -1.0, 0.0);
                 st_s.packed += 1; st_s.ep_len += 1;
                 st_s.vol_sum += vol_pf;
                 st_s.ep_rew += rew;
@@ -716,16 +733,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
                 for (int q = oa; q + 1 < nfill; ++q) queue_g[q] = queue_g[q + 1];
                 queue_g[nfill - 1] = draw();
             } else {
-                P.r_reward[env] = 0.0f; P.r_done[env] = 1; P.r_valid[env] = 1;
-                P.r_counter[env] = st_s.packed;
-                P.r_ratio[env] = st_s.vol_sum / P.binvol;
-                P.r_eplen[env] = st_s.ep_len + 1;
-                P.r_eprew[env] = st_s.ep_rew + 0.0;
-                if (P.h_reward) {
-                    P.h_reward[env] = 0.0f; P.h_done[env] = 1; P.h_valid[env] = 1;
-                    P.h_counter[env] = st_s.packed; P.h_ratio[env] = st_s.vol_sum / P.binvol;
-                    P.h_eplen[env] = st_s.ep_len + 1; P.h_eprew[env] = st_s.ep_rew + 0.0;
-                }
+                store_results(P, env, 0.0f, 1, 1, st_s.packed, st_s.ep_len + 1, st_s.vol_sum / P.binvol, st_s.ep_rew + 0.0);
                 st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0;
                 st_s.order_act = 0;
                 live = new_episode();
@@ -765,7 +773,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         const int width = emit_loc ? P.loc_len : P.order_len;
         for (int i = tid; i < width; i += CTA_THREADS) obs_g[i] = 0.0f;
         if (tid == 0) {
-            if (mode != MODE_ALL_OBS) { P.r_error[env] = (uint8_t)err_sh; if (P.h_error) P.h_error[env] = (uint8_t)err_sh; }
+            if (mode != MODE_ALL_OBS) store_error(P, env, err_sh);
             st_s.next_seq = next_seq;
         }
         __syncthreads();
@@ -786,7 +794,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     if (!emit_loc) {
         // order observation: [next k item ids | heightmap]  (binPhy.py:229-230)
         for (int i = tid; i < P.K; i += CTA_THREADS) obs_g[i] = (float)queue_g[i];
-        if (tid == 0) { P.r_error[env] = (uint8_t)err_sh; if (P.h_error) P.h_error[env] = (uint8_t)err_sh; st_s.next_seq = next_seq; }
+        if (tid == 0) { store_error(P, env, err_sh); st_s.next_seq = next_seq; }
         if (st_dirty && warp == 0) {
             __syncwarp();
             reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st_s)[lane];
@@ -835,10 +843,9 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
     }
     __syncthreads();
     if (tid == 0) {
-        if (mode != MODE_ALL_OBS || err_sh) {      // (several CTAs per bin in MODE_ALL_OBS: only error codes are written)
-            P.r_error[env] = (uint8_t)err_sh;      // the candidates kernel may overwrite with its own code
-            if (P.h_error) P.h_error[env] = (uint8_t)err_sh;
-        }
+        // (several CTAs per bin in MODE_ALL_OBS: only error codes are written; the candidates kernel may overwrite
+        // with its own code)
+        if (mode != MODE_ALL_OBS || err_sh) store_error(P, env, err_sh);
         const bool write_state = (mode == MODE_STEP || mode == MODE_RESET || mode == MODE_CANDIDATES ||
                                   (mode == MODE_ALL_OBS && slot == P.K - 1));
         if (write_state) { st_s.cur_item = item; st_s.mask_any = any_sh; }
@@ -890,7 +897,7 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_levels_kernel(const Params 
     }
     if (err) err_sh = 4;
     __syncthreads();
-    if (threadIdx.x == 0) P.r_error[env] = (uint8_t)err_sh;
+    if (threadIdx.x == 0) P.res.error[env] = (uint8_t)err_sh;
 }
 
 // ---- heuristic kernel (space.py:162-227) ---------------------------------------------------------------------
@@ -1522,7 +1529,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         if (Ktot < sel) zero_rows(Ktot);
     }
     if (lane == 0) {
-        if (dev_err) { P.r_error[renv] = (uint8_t)dev_err; if (P.h_error) P.h_error[renv] = (uint8_t)dev_err; }
+        if (dev_err) store_error(P, renv, dev_err);
         if (P.dbg_nhull) P.dbg_nhull[env] = Ktot;
     }
     if (warp == 0) trace(6);

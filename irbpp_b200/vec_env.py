@@ -110,9 +110,6 @@ class LazyInfos(Sequence):
     when indexed (at N = 4096 eagerly building them would dominate the step).  Holds this step's private
     copy of the library's result block; the typed views are cut out of it on first use."""
 
-    _FIELDS = (("valid", np.bool_), ("counter", np.int32), ("ratio", np.float64),
-               ("ep_reward", np.float64), ("ep_len", np.int32))
-
     def __init__(self, n, block, offsets, done, t_rel, borrowed=False):
         self._n, self._block, self._offsets, self._done, self._t = n, block, offsets, done, t_rel
         self._v = None
@@ -129,7 +126,8 @@ class LazyInfos(Sequence):
     def _views(self):
         if self._v is None:
             n, b, o = self._n, self._block, self._offsets
-            self._v = {k: b[o[k]:o[k] + n * np.dtype(dt).itemsize].view(dt) for k, dt in self._FIELDS}
+            self._v = {k: b[o[k]:o[k] + n * dt.itemsize].view(np.bool_ if k == "valid" else dt)
+                       for k, dt in _lib.RESULT_FIELDS}
         return self._v
 
     def __len__(self):
@@ -395,9 +393,6 @@ class GpuVecEnv(VecEnv):
             if old is not None:
                 old.detach()
 
-    _RESULT_BYTES = (("ratio", 8), ("ep_reward", 8), ("reward", 4), ("counter", 4), ("ep_len", 4),
-                     ("done", 1), ("valid", 1), ("error", 1))
-
     def _result_block(self, res):
         """uint8 view of the library's pinned result block and the byte offset of every array in it (from
         the pointers of ``irbpp_step_result``; two blocks per handle, each view built once)."""
@@ -406,11 +401,11 @@ class GpuVecEnv(VecEnv):
         hit = cache.get(key)
         if hit is None:
             n = self.num_envs
-            ptrs = {k: getattr(res, k) for k, _ in self._RESULT_BYTES}
+            ptrs = {k: getattr(res, k) for k, _ in _lib.RESULT_FIELDS}
             base = min(ptrs.values())
-            end = max(ptrs[k] + n * sz for k, sz in self._RESULT_BYTES)
+            end = max(ptrs[k] + n * dt.itemsize for k, dt in _lib.RESULT_FIELDS)
             buf = (ctypes.c_uint8 * (end - base)).from_address(base)
-            hit = cache[key] = (np.frombuffer(buf, dtype=np.uint8), {k: ptrs[k] - base for k, _ in self._RESULT_BYTES})
+            hit = cache[key] = (np.frombuffer(buf, dtype=np.uint8), {k: p - base for k, p in ptrs.items()})
         return hit
 
     def step_device(self, actions):
@@ -430,9 +425,10 @@ class GpuVecEnv(VecEnv):
         return obs, res
 
     def last_step_device(self):
-        """Device views of the last step's result arrays -- ``reward`` float32 [N], ``done`` / ``valid`` uint8 [N],
-        ``counter`` int32 [N], ``ratio`` float64 [N] -- as torch tensors aliasing the library's buffers (valid until
-        the next step on this handle): what a device-resident replay bank appends without any host round trip."""
+        """Device views of the last step's result arrays -- every field of ``_lib.RESULT_FIELDS``, e.g. ``reward``
+        float32 [N], ``done`` / ``valid`` uint8 [N], ``counter`` int32 [N], ``ratio`` float64 [N] -- as torch tensors
+        aliasing the library's buffers (valid until the next step on this handle): what a device-resident replay bank
+        appends without any host round trip."""
         torch = self._torch
         views = getattr(self, "_dev_views", None)
         if views is None:                             # the device arrays are fixed for the life of the handle: built once
@@ -443,9 +439,8 @@ class GpuVecEnv(VecEnv):
             class _View(object):
                 def __init__(self, ptr, shape, typestr):
                     self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr), False), "version": 2}
-            spec = {"reward": "<f4", "done": "|u1", "valid": "|u1", "counter": "<i4", "ratio": "<f8", "ep_len": "<i4", "ep_reward": "<f8"}
-            views = self._dev_views = {k: torch.as_tensor(_View(getattr(res, k), (n,), ts), device=self.device)
-                                       for k, ts in spec.items()}
+            views = self._dev_views = {k: torch.as_tensor(_View(getattr(res, k), (n,), dt.str), device=self.device)
+                                       for k, dt in _lib.RESULT_FIELDS}
         return views
 
     def get_action_candidates(self, order_actions, as_tensor=False):

@@ -10,12 +10,10 @@ from irbpp_b200.vec_env import GpuVecEnv, LazyInfos
 
 def _fake_result(n):
     """A host buffer laid out like the library's pinned result block (include/irbpp.h, irbpp_step_result)."""
-    sizes = (("ratio", 8), ("ep_reward", 8), ("reward", 4), ("counter", 4), ("ep_len", 4), ("done", 1),
-             ("valid", 1), ("error", 1))
     offs, o = {}, 0
-    for k, sz in sizes:
+    for k, dt in _lib.RESULT_FIELDS:
         offs[k] = o
-        o += sz * n
+        o += dt.itemsize * n
     buf = np.zeros(o + 16, np.uint8)
     res = _lib.IrbppStepResult()
     for k in offs:

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 from conftest import load_golden
+from irbpp_b200 import _lib
 from test_kernels_emulated import EmuEnv, build_emulated
 
 pytestmark = pytest.mark.timeout(900)
@@ -77,10 +78,6 @@ def emu(tmp_path_factory):
     return build_emulated(str(tmp_path_factory.mktemp("emu_items")))
 
 
-class _Res(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_void_p) for n in ("reward", "done", "valid", "error", "counter", "ep_len", "ratio", "ep_reward")]
-
-
 class ItemEnv(EmuEnv):
     """EmuEnv whose item source is replaced by groups or trajectories; step() also returns Valid."""
 
@@ -99,7 +96,7 @@ class ItemEnv(EmuEnv):
         acts = np.ascontiguousarray(actions, dtype=np.int64)
         obs = np.zeros((self.n, self.obs_len), np.float32)
         assert self.lib.emu_irbpp_step_async(self.h, _P(acts), 0, _P(obs), None) == 0
-        res = _Res()
+        res = _lib.IrbppStepResult()
         rc = self.lib.emu_irbpp_step_wait(self.h, ctypes.byref(res))
         view = lambda p, ct, dt: np.frombuffer((ct * self.n).from_address(p), dtype=dt).copy()
         out = {k: view(getattr(res, k), ct, dt) for k, ct, dt in (

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 from conftest import lib_from_fixture, load_golden
+from irbpp_b200 import _lib
 
 pytestmark = pytest.mark.timeout(900)          # a deadlocked emulated barrier must not hang the suite
 
@@ -62,23 +63,12 @@ def emu(tmp_path_factory):
     return build_emulated(str(tmp_path_factory.mktemp("emu")))
 
 
-class _Cfg(ctypes.Structure):
-    _fields_ = [("num_envs", ctypes.c_int32), ("num_rotations", ctypes.c_int32), ("selected_action", ctypes.c_int32),
-                ("buffer_size", ctypes.c_int32), ("bin_dimension", ctypes.c_double * 3), ("resolution_act", ctypes.c_double),
-                ("resolution_h", ctypes.c_double), ("resolution_z", ctypes.c_double), ("device", ctypes.c_int32),
-                ("approx_legacy", ctypes.c_int32)]
-
-
-class _Res(ctypes.Structure):
-    _fields_ = [(n, ctypes.c_void_p) for n in ("reward", "done", "valid", "error", "counter", "ep_len", "ratio", "ep_reward")]
-
-
 class EmuEnv(object):
     """The C ABI of include/irbpp.h driven with NumPy buffers (device == host under the emulation)."""
 
     def __init__(self, lib, library, sequences, selected_action=500, buffer_size=1):
         self.lib, self.n = lib, len(sequences)
-        cfg = _Cfg(self.n, library.num_rotations, selected_action, buffer_size, (ctypes.c_double * 3)(0.32, 0.32, 0.30),
+        cfg = _lib.IrbppConfig(self.n, library.num_rotations, selected_action, buffer_size, (ctypes.c_double * 3)(0.32, 0.32, 0.30),
                    0.02, 0.01, 0.01, 0, 0)
         self.h = ctypes.c_void_p()
         assert lib.emu_irbpp_create(ctypes.byref(cfg), ctypes.byref(self.h)) == 0
@@ -98,15 +88,22 @@ class EmuEnv(object):
         assert self.lib.emu_irbpp_reset(self.h, None, ctypes.c_void_p(obs.ctypes.data), None) == 0
         return obs
 
-    def step(self, actions):
+    def step_results(self, actions, on_device=0):
+        """-> (obs, {field: copy of its array} for every field of _lib.RESULT_FIELDS).  ``on_device = 1`` passes the
+        actions as device actions (device == host here): the kernels then store the results only into the device
+        block, which irbpp_step_wait copies back."""
         acts = np.ascontiguousarray(actions, dtype=np.int64)
         obs = np.zeros((self.n, self.obs_len), np.float32)
-        assert self.lib.emu_irbpp_step_async(self.h, ctypes.c_void_p(acts.ctypes.data), 0, ctypes.c_void_p(obs.ctypes.data), None) == 0
-        res = _Res()
+        assert self.lib.emu_irbpp_step_async(self.h, ctypes.c_void_p(acts.ctypes.data), on_device,
+                                             ctypes.c_void_p(obs.ctypes.data), None) == 0
+        res = _lib.IrbppStepResult()
         assert self.lib.emu_irbpp_step_wait(self.h, ctypes.byref(res)) == 0, self.lib.emu_irbpp_last_error(self.h)
-        view = lambda p, ct, dt: np.frombuffer((ct * self.n).from_address(p), dtype=dt).copy()
-        return (obs, view(res.reward, ctypes.c_float, np.float32), view(res.done, ctypes.c_uint8, np.bool_),
-                view(res.counter, ctypes.c_int32, np.int32), view(res.ratio, ctypes.c_double, np.float64))
+        return obs, {k: np.frombuffer((ctypes.c_uint8 * (self.n * dt.itemsize)).from_address(getattr(res, k)), dtype=dt).copy()
+                     for k, dt in _lib.RESULT_FIELDS}
+
+    def step(self, actions):
+        obs, r = self.step_results(actions)
+        return obs, r["reward"], r["done"].view(np.bool_), r["counter"], r["ratio"]
 
     def get_action_candidates(self, order):
         order = np.ascontiguousarray(order, dtype=np.int64)
@@ -145,6 +142,27 @@ def _replay(lib, name, steps):
                                         ("episode_truncate", 6), ("episode_buffered", 6), ("episode_buffered10", 5), ("episode_rot24", 3)])
 def test_emulated_kernels_replay_reference_episodes(emu, name, steps):
     _replay(emu, name, steps)
+
+
+def test_emulated_host_and_device_result_blocks_agree(emu):
+    """A step's results reach the host through the host-mapped block (host actions) or through the device block that
+    irbpp_step_wait copies back (device actions).  A golden episode played both ways gives the same arrays at every
+    step, auto-resets included."""
+    d = load_golden("episode_cube")
+    envs = [EmuEnv(emu, lib_from_fixture(d), d["sequences"]) for _ in range(2)]
+    for env in envs:
+        env.reset()
+    dones = 0
+    for t in range(14):
+        (obs0, res0), (obs1, res1) = [env.step_results(d["actions"][t], on_device=i) for i, env in enumerate(envs)]
+        assert np.array_equal(obs0, obs1), t
+        for k, _ in _lib.RESULT_FIELDS:
+            assert np.array_equal(res0[k], res1[k]), (k, t)
+        assert np.array_equal(res0["reward"], d["reward"][t].astype(np.float32)), t
+        dones += int(res0["done"].sum())
+    assert dones > 0
+    for env in envs:
+        env.close()
 
 
 
