@@ -12,8 +12,6 @@ DEPS = sorted(glob.glob(os.path.join(HERE, "csrc", "*.cu")) + glob.glob(os.path.
     [os.path.join(ROOT, "include", "irbpp.h"), os.path.abspath(__file__)]
 OUT_DIR = os.path.join(HERE, "lib")
 OUT = os.path.join(OUT_DIR, "libirbpp.so")
-# experiment hook: extra -D flags and an alternative output name (IRBPP_LIB selects it at load time)
-EXTRA_DEFS = os.environ.get("IRBPP_BUILD_DEFS", "").split()
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-fmad=false",                      # float64 must round exactly like NumPy: no FMA contraction
@@ -34,15 +32,15 @@ def up_to_date():
     return all(os.path.getmtime(d) <= t for d in DEPS)
 
 
-def build(force=False, verbose=False, out=None, defs=None):
-    """Compile ``csrc/irbpp.cu`` -> ``lib/libirbpp.so`` (nvcc cross-compiles without a GPU)."""
-    defs = EXTRA_DEFS if defs is None else defs
+def build(force=False, verbose=False, out=None):
+    """Compile ``csrc/irbpp.cu`` -> ``lib/libirbpp.so`` (nvcc cross-compiles without a GPU).  ``out``: another path for
+    the library, e.g. to time two builds against each other (``IRBPP_LIB`` selects one at load time)."""
     if out is None:
         out = OUT
-        if not force and not defs and up_to_date():
+        if not force and up_to_date():
             return OUT
     os.makedirs(OUT_DIR, exist_ok=True)
-    cmd = [nvcc_path()] + NVCC_FLAGS + list(defs) + (["-Xptxas", "-v"] if verbose else []) + ["-o", out, SRC]
+    cmd = [nvcc_path()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", out, SRC]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose:
         sys.stderr.write(res.stderr)

@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <functional>
+#include <map>
 #include <mutex>
 #include <cmath>
 #include <string>
@@ -29,7 +30,7 @@ static thread_local std::string g_create_error;     // error of the calling thre
 struct irbpp_env {
     irbpp_config cfg;
     Params P;                      // device pointers + configuration (mode/inputs filled per launch)
-    int cand_smem = 0, scan_smem = 0;
+    int scan_smem = 0;
     uint32_t* ready_dev = nullptr;       // scan -> candidates hand-over flags (one per unit)
     uint32_t epoch = 0;                  // launch counter behind the flags
     int epc = ENVS_PER_CTA_NARROW;       // bins per CTA of the candidates kernel (envs_per_cta_for(R))
@@ -152,30 +153,35 @@ static void free_dev(irbpp_env* h, void* p) {
     cudaFree(p);
 }
 
+// The step kernels of a configuration: `epc` bins per candidates CTA (envs_per_cta_for(R)), `traj`: the trajectory
+// item source, and the candidates kernel's dynamic shared memory at R rotations.
+struct StepKernels {
+    void (*scan)(const Params);
+    void (*cand)(const Params);
+    int cand_smem;
+};
+
+template <int EPC>
+static StepKernels step_kernels_epc(bool traj, int R) {
+    return {traj ? irbpp_scan_kernel<true> : irbpp_scan_kernel<false>,
+            traj ? irbpp_candidates_kernel<EPC, true> : irbpp_candidates_kernel<EPC, false>, cand_smem_bytes<EPC>(R)};
+}
+
+static StepKernels step_kernels(int epc, bool traj, int R) {
+    return epc == ENVS_PER_CTA_WIDE ? step_kernels_epc<ENVS_PER_CTA_WIDE>(traj, R) : step_kernels_epc<ENVS_PER_CTA_NARROW>(traj, R);
+}
+
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-function, PER-DEVICE attribute: the largest value any
-// handle needed is tracked per device ordinal and only ever raised (several handles may coexist on a device,
-// and one process may hold handles on several devices).  which: 0 / 3 candidates kernel (narrow / wide CTA), 1 scan kernel, 2 shape encoder.
-static cudaError_t raise_dynamic_smem(int device, int which, int bytes) {
-    static int raised[64][4];
+// handle needed is tracked per (device, kernel) and only ever raised (several handles may coexist on a device,
+// and one process may hold handles on several devices).
+static cudaError_t raise_dynamic_smem(int device, const void* kernel, int bytes) {
+    static std::map<std::pair<int, const void*>, int> raised;
     static std::mutex mu;
     std::lock_guard<std::mutex> lk(mu);
-    if (device < 0 || device >= 64) return cudaErrorInvalidDevice;
-    if (bytes <= raised[device][which]) return cudaSuccess;
-    const cudaFuncAttribute a = cudaFuncAttributeMaxDynamicSharedMemorySize;
-    cudaError_t e = cudaSuccess;
-    if (which == 0) {
-        e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, false>, a, bytes);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, true>, a, bytes);
-    } else if (which == 3) {
-        e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, false>, a, bytes);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, true>, a, bytes);
-    } else if (which == 1) {
-        e = cudaFuncSetAttribute(irbpp_scan_kernel<false>, a, bytes);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(irbpp_scan_kernel<true>, a, bytes);
-    } else {
-        e = cudaFuncSetAttribute(irbpp_shape_encode_kernel, a, bytes);
-    }
-    if (e == cudaSuccess) raised[device][which] = bytes;
+    int& done = raised[{device, kernel}];
+    if (bytes <= done) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) done = bytes;
     return e;
 }
 
@@ -237,7 +243,6 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     P.resA = cfg->resolution_act;
     P.binvol = (cfg->bin_dimension[0] * cfg->bin_dimension[1]) * cfg->bin_dimension[2];   // np.prod
     h->epc = envs_per_cta_for(P.R);                  // bins (= warps) per CTA of the candidates kernel
-    h->cand_smem = h->epc == ENVS_PER_CTA_WIDE ? cand_smem_bytes<ENVS_PER_CTA_WIDE>(P.R) : cand_smem_bytes<ENVS_PER_CTA_NARROW>(P.R);
 
 #define TRY_ALLOC(expr)                                                                          \
     do { cudaError_t e2_ = (expr); if (e2_ != cudaSuccess) {                                      \
@@ -266,7 +271,10 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     }
     TRY_ALLOC(cudaHostAlloc((void**)&h->actions_pinned, 2 * (size_t)N * sizeof(int64_t), cudaHostAllocMapped));
     P.res = step_results(h->results_dev, N);
-    TRY_ALLOC(raise_dynamic_smem(cfg->device, h->epc == ENVS_PER_CTA_WIDE ? 3 : 0, h->cand_smem));
+    for (bool traj : {false, true}) {
+        const StepKernels k = step_kernels(h->epc, traj, P.R);
+        TRY_ALLOC(raise_dynamic_smem(cfg->device, (const void*)k.cand, k.cand_smem));
+    }
 #undef TRY_ALLOC
     *out = h;
     return IRBPP_OK;
@@ -302,7 +310,7 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
     std::vector<double> Bs, Ts;
     std::vector<TileEntry> tiles;
     std::vector<double> rew(S);
-    int maxwh = 1, max_entries = 1;
+    int max_entries = 1;
     for (int s = 0; s < S; ++s) {
         rew[s] = (vol[s] / h->P.binvol) * 10;                        // binPhy.py:155-156,321-322
         for (int r = 0; r < R; ++r) {
@@ -317,7 +325,6 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
                             "(the reference fails on this table)", s, r, w, hh, wA, hA);
             const int64_t off = offsets[(size_t)s * R + r];
             const int64_t n = (int64_t)w * hh;
-            if ((int)n > maxwh) maxwh = (int)n;
             if (off < 0 || off + 4 * n > maps_len) return fail(h, IRBPP_EINVAL, "shape %d rot %d: table out of range", s, r);
             ShapeRot& q = srot[(size_t)s * R + r];
             q.w = w; q.h = hh;
@@ -418,11 +425,11 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
     CUDA_TRY(h, cudaMemcpy(h->rew_dev, rew.data(), (size_t)S * 8, cudaMemcpyHostToDevice));
     h->P.S = S; h->P.srot = h->srot_dev; h->P.Bs = h->Bs_dev; h->P.Ts = h->Ts_dev;
     h->P.vol = h->vol_dev; h->P.reward_tab = h->rew_dev;
-    (void)maxwh;
     h->P.maxwh = max_entries;
     // per-warp staging lists, then the bin's candidate table row (bulk-copied by the scan kernel)
     h->scan_smem = CTA_WARPS * h->P.maxwh * (int)sizeof(TileEntry) + ((h->P.cand_stride * 2 + 15) & ~15);
-    CUDA_TRY(h, raise_dynamic_smem(c.device, 1, h->scan_smem));
+    for (bool traj : {false, true})
+        CUDA_TRY(h, raise_dynamic_smem(c.device, (const void*)step_kernels(h->epc, traj, h->P.R).scan, h->scan_smem));
     h->shapes_loaded = true;
     return IRBPP_OK;
 }
@@ -549,44 +556,38 @@ int irbpp_set_trajectories(irbpp_handle h, const int32_t* items, const int64_t* 
 // candidates kernel when the observation carries candidate rows.  (Running bin ranges on separate
 // streams so that one range's candidates kernel overlaps the next range's scan kernel was measured:
 // no gain -- the scan kernel owns the whole register file, the two cannot co-reside.)
-// IRBPP_HANDOVER=grid restores the grid-wide wait (measurement switch)
-static bool flags_enabled() {
-    static const bool on = [] { const char* e = getenv("IRBPP_HANDOVER"); return !(e && strcmp(e, "grid") == 0); }();
-    return on;
-}
 
 static int launch(irbpp_env* h, Params& P, cudaStream_t s) {
     // the units of a launch: bins, or (bin, buffer slot) pairs for get_all_possible_observation
     const int units = (P.mode == MODE_ALL_OBS) ? P.N * P.K : P.N;
     P.env_lo = 0;
     P.env_hi = units;
-    // per-unit hand-over flags instead of the grid-wide dependency wait.  Not for caller-supplied maps (the levels kernel
-    // sets none) and not for the fused all-slot pass (the k scan CTAs of a bin share its state and candidate table, which
-    // the candidates CTA of the last slot rewrites: that one must wait for all of them)
-    P.ready = (P.mode == MODE_DEBUG_HULLS || P.mode == MODE_ALL_OBS || !flags_enabled()) ? nullptr : h->ready_dev;
+    const bool cand_follows = mode_emits_loc(P.mode, P.K);
+    // per-unit hand-over flags instead of the grid-wide dependency wait, whenever a candidates grid follows.  Not for
+    // caller-supplied maps (the levels kernel sets none) and not for the fused all-slot pass (the k scan CTAs of a bin
+    // share its state and candidate table, which the candidates CTA of the last slot rewrites: that one must wait for all
+    // of them)
+    P.ready = (cand_follows && P.mode != MODE_DEBUG_HULLS && P.mode != MODE_ALL_OBS) ? h->ready_dev : nullptr;
     if (++h->epoch == 0) h->epoch = 1;
     P.epoch = h->epoch;
+    const StepKernels k = step_kernels(h->epc, P.item_src == ITEMS_TRAJ, P.R);
     if (P.mode == MODE_DEBUG_HULLS) irbpp_levels_kernel<<<P.N, CTA_THREADS, 0, s>>>(P);
     else {
-        void (*scan)(const Params) = P.item_src == ITEMS_TRAJ ? irbpp_scan_kernel<true> : irbpp_scan_kernel<false>;
+        void (*scan)(const Params) = k.scan;
         scan<<<units, CTA_THREADS, h->scan_smem, s>>>(P);
     }
     h->launches += 1;
-    if (mode_emits_loc(P.mode, P.K)) {
+    if (cand_follows) {
         // programmatic dependent launch: the candidates grid is scheduled while the scan grid's last
         // wave drains and waits at griddepcontrol.wait for the scan's completion
         cudaLaunchConfig_t lc = {};
         lc.gridDim = dim3((units + h->epc - 1) / h->epc); lc.blockDim = dim3(32 * h->epc);
-        lc.dynamicSmemBytes = (size_t)h->cand_smem; lc.stream = s;
+        lc.dynamicSmemBytes = (size_t)k.cand_smem; lc.stream = s;
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = (P.mode == MODE_DEBUG_HULLS) ? 0 : 1;
         lc.attrs = at; lc.numAttrs = 1;
-        const bool traj = P.item_src == ITEMS_TRAJ;
-        void (*cand)(const Params) = h->epc == ENVS_PER_CTA_WIDE
-            ? (traj ? irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, true> : irbpp_candidates_kernel<ENVS_PER_CTA_WIDE, false>)
-            : (traj ? irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, true> : irbpp_candidates_kernel<ENVS_PER_CTA_NARROW, false>);
-        cudaLaunchKernelEx(&lc, cand, P);
+        cudaLaunchKernelEx(&lc, k.cand, P);
         h->launches += 1;
     }
     cudaError_t e = cudaGetLastError();
@@ -933,7 +934,7 @@ int irbpp_shape_features(const float* shape_array, int32_t S, int32_t P, const f
     Q.W1 = W1; Q.b1 = b1; Q.W2 = W2; Q.b2 = b2; Q.slope = negative_slope; Q.feat_keys = scratch_keys; Q.out = out;
     const int dev = device_of(shape_array);
     DeviceGuard guard(dev);
-    cudaError_t e = raise_dynamic_smem(dev, 2, PN_SMEM_BYTES);
+    cudaError_t e = raise_dynamic_smem(dev, (const void*)irbpp_shape_encode_kernel, PN_SMEM_BYTES);
     if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "shape encoder set-up: %s", cudaGetErrorString(e));
     cudaStream_t s = (cudaStream_t)stream;
     irbpp_pn_init_kernel<<<(S * PN_H + 255) / 256, 256, 0, s>>>(scratch_keys, S * PN_H);
@@ -1026,22 +1027,10 @@ int irbpp_replay_update_priorities(const irbpp_replay_memory* mem, const int32_t
 int irbpp_debug_phase_cycles(irbpp_handle h, int32_t enable, uint64_t* out8) {
     if (!h) return IRBPP_EINVAL;
     DeviceGuard guard(h->cfg.device);
-#ifdef IRBPP_PROBE_TRACE
-    const size_t trace_words = 8 + ((size_t)h->P.N * h->P.K + 1) * 8;     // profiling build: per-CTA timelines behind the counters
-#else
-    const size_t trace_words = 8;
-#endif
-    if (!h->phase_dev) CUDA_TRY(h, dev_alloc(h, &h->phase_dev, trace_words));
+    if (!h->phase_dev) CUDA_TRY(h, dev_alloc(h, &h->phase_dev, 8));
     CUDA_TRY(h, cudaDeviceSynchronize());
     if (out8) CUDA_TRY(h, cudaMemcpy(out8, h->phase_dev, 8 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-#ifdef IRBPP_PROBE_TRACE
-    if (const char* path = getenv("IRBPP_TRACE_FILE")) {
-        std::vector<unsigned long long> tr(trace_words);
-        CUDA_TRY(h, cudaMemcpy(tr.data(), h->phase_dev, trace_words * 8, cudaMemcpyDeviceToHost));
-        if (FILE* f = fopen(path, "wb")) { fwrite(tr.data(), 8, trace_words, f); fclose(f); }
-    }
-#endif
-    CUDA_TRY(h, cudaMemset(h->phase_dev, 0, trace_words * sizeof(uint64_t)));
+    CUDA_TRY(h, cudaMemset(h->phase_dev, 0, 8 * sizeof(uint64_t)));
     h->P.phase_cycles = enable ? h->phase_dev : nullptr;
     return IRBPP_OK;
 }

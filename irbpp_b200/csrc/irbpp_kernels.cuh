@@ -51,23 +51,12 @@ constexpr int CTA_WARPS = CTA_THREADS / 32;
 // Timed on an H100 SXM (700 W) with the earlier 4 KB warp scratch, ms per step of 4096 bins: BlockOut R = 4  0.147 with 4 bins /
 // 0.158 with 8; irregular R = 8 and R = 24 within noise with 6, 7 or 8 (0.373-0.379, 2.55-2.57) -- with many rotations a CTA's
 // fixed phases amortise over more images and the task deal balances over 256 lanes.
-#ifndef IRBPP_ENVS_PER_CTA
-#define IRBPP_ENVS_PER_CTA 4
-#endif
-#ifndef IRBPP_ENVS_PER_CTA_WIDE
-#define IRBPP_ENVS_PER_CTA_WIDE 8
-#endif
-#ifndef IRBPP_WIDE_MIN_R
-#define IRBPP_WIDE_MIN_R 8
-#endif
-constexpr int ENVS_PER_CTA_NARROW = IRBPP_ENVS_PER_CTA;
-constexpr int ENVS_PER_CTA_WIDE = IRBPP_ENVS_PER_CTA_WIDE;
-__host__ __device__ inline int envs_per_cta_for(int R) { return R >= IRBPP_WIDE_MIN_R ? ENVS_PER_CTA_WIDE : ENVS_PER_CTA_NARROW; }
+constexpr int ENVS_PER_CTA_NARROW = 4, ENVS_PER_CTA_WIDE = 8;
+constexpr int WIDE_MIN_R = 8;
+__host__ __device__ inline int envs_per_cta_for(int R) { return R >= WIDE_MIN_R ? ENVS_PER_CTA_WIDE : ENVS_PER_CTA_NARROW; }
 constexpr int MAX_LEVELS = 64;           // level-image slots per (bin, rotation) in the scratch
-#ifndef IRBPP_TASKS_PER_LANE
-#define IRBPP_TASKS_PER_LANE 2
-#endif
-constexpr int TASKS_PER_LANE = IRBPP_TASKS_PER_LANE;        // micro-tasks a lane takes per batch of the candidates kernel (one follow / sort / approximate cycle)
+constexpr int TASKS_PER_LANE = 2;        // micro-tasks a lane takes per batch of the candidates kernel (one follow / sort / approximate cycle)
+constexpr int SCAN_MIN_CTAS = 8;         // scan CTAs per SM the scan kernel is built for (64 registers per thread)
 constexpr int TASK_TAB = 384;            // start pixels of a round listed explicitly (the rest are found by search)
 constexpr int FAST_CAP = 64;             // contour points on the fast path (32 was measured slower: every overflow redo stalls a warp)
 constexpr int BIG_CAP = 1024;            // contour points on the overflow path
@@ -305,11 +294,68 @@ __host__ __device__ __forceinline__ bool mode_emits_loc(int mode, int K) {
     return !((mode == MODE_STEP || mode == MODE_RESET) && K > 1);
 }
 
-// ---- level bitmaps of one rotation -------------------------------------------------------------------
-// lv[pass] = level of pose pass*32+lane (or -1).  One 16x16 bitmap (8 words, two rows each) per level
-// present, by warp ballots, written to the scratch; returns the number of levels.
-__device__ __forceinline__ int emit_level_bitmaps(uint32_t* bm_g, int lane, const int (&lv)[8], uint64_t present) {
+// Whether a call's pass over buffer slot `slot` owns the bin's scalar state and candidate table: every call that changes
+// the bin's current item, and of the K passes of get_all_possible_observation the last one.
+__host__ __device__ __forceinline__ bool mode_writes_state(int mode, int slot, int K) {
+    return mode == MODE_STEP || mode == MODE_RESET || mode == MODE_CANDIDATES || (mode == MODE_ALL_OBS && slot == K - 1);
+}
+
+// ---- scan -> candidates scratch: the slice of unit u (a bin, or a (bin, buffer slot) pair) and rotation r ----------
+__device__ __forceinline__ double* posz_of(const Params& P, int u, int r) { return P.posz + ((int64_t)u * P.R + r) * NPOSE; }
+__device__ __forceinline__ uint32_t* maskbits_of(const Params& P, int u, int r) { return P.maskbits + ((int64_t)u * P.R + r) * 8; }
+__device__ __forceinline__ uint32_t* bitmaps_of(const Params& P, int u, int r) { return P.bitmaps + ((int64_t)u * P.R + r) * MAX_LEVELS * 8; }
+__device__ __forceinline__ int32_t* nlevels_of(const Params& P, int u, int r) { return P.nlevels + (int64_t)u * P.R + r; }
+
+// ---- warp and phase helpers of both step kernels ----------------------------------------------------------------
+__device__ __forceinline__ int warp_inclusive_scan(int v, int lane) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += t; }
+    return v;
+}
+
+// one warp: exclusive prefix of 64 bucket counts
+__device__ __forceinline__ void bucket_prefix64(const int32_t* hist, int32_t* hbase, int lane) {
+    const int h0 = hist[lane], h1 = hist[32 + lane];
+    const int i0 = warp_inclusive_scan(h0, lane), i1 = warp_inclusive_scan(h1, lane);
+    const int tot0 = __shfl_sync(0xffffffffu, i0, 31);
+    hbase[lane] = i0 - h0;
+    hbase[32 + lane] = tot0 + i1 - h1;
+}
+
+// Per-phase SM cycles (irbpp_debug_phase_cycles): thread 0 of a CTA adds the cycles since its previous mark to counter `idx`.
+// `t` holds thread 0's previous mark; the scan kernel keeps it in shared memory, so that no thread carries it in registers
+// through phase B.
+struct PhaseClock {
+    const Params& P;
+    long long& t_prev;
+    __device__ __forceinline__ PhaseClock(const Params& p, long long& t) : P(p), t_prev(t) { if (P.phase_cycles && threadIdx.x == 0) t_prev = clock64(); }
+    __device__ __forceinline__ void mark(int idx) {
+        if (P.phase_cycles && threadIdx.x == 0) {
+            const long long now = clock64();
+            atomicAdd(P.phase_cycles + idx, (unsigned long long)(now - t_prev));
+            t_prev = now;
+        }
+    }
+};
+
+// ---- level images of one rotation -------------------------------------------------------------------
+// presence bit of level L in [-32, 31]
+__device__ __forceinline__ void mark_level(int L, uint32_t& pres_lo, uint32_t& pres_hi) {
+    if (L != -1) {
+        const int b = L + LEVEL_OFFSET;
+        if (b < 32) pres_lo |= 1u << b; else pres_hi |= 1u << (b - 32);
+    }
+}
+
+// lv[pass] = level of pose pass*32+lane (or -1), pres_lo / pres_hi = this lane's presence bits.  One 16x16 bitmap (8
+// words, two rows each) per level present in the warp, by warp ballots, written to the scratch with their count.
+__device__ __forceinline__ void emit_level_bitmaps(const Params& P, int u, int r, int lane, const int (&lv)[8],
+                                                   uint32_t pres_lo, uint32_t pres_hi) {
+    pres_lo = __reduce_or_sync(0xffffffffu, pres_lo);
+    pres_hi = __reduce_or_sync(0xffffffffu, pres_hi);
+    uint64_t present = ((uint64_t)pres_hi << 32) | pres_lo;
     present &= ~(1ull << (LEVEL_OFFSET - 1));        // level -1 is skipped (cvTools.py:84)
+    uint32_t* bm_g = bitmaps_of(P, u, r);
     int k = 0;
     while (present) {
         const int b = __ffsll((long long)present) - 1;
@@ -324,17 +370,14 @@ __device__ __forceinline__ int emit_level_bitmaps(uint32_t* bm_g, int lane, cons
         if (lane < 8) bm_g[k * 8 + lane] = mine;
         ++k;
     }
-    return k;
+    if (lane == 0) *nlevels_of(P, u, r) = k;
 }
 
 __device__ __forceinline__ int level_of(const Params& P, double posz, double inv, uint32_t& pres_lo,
                                         uint32_t& pres_hi, int& err) {
     int L = (int)floor_divide_exact(posz, P.resZ, inv);        // cvTools.py:78
     if (L < -LEVEL_OFFSET || L >= LEVEL_OFFSET) { err = 1; return -1; }
-    if (L != -1) {
-        const int b = L + LEVEL_OFFSET;
-        if (b < 32) pres_lo |= 1u << b; else pres_hi |= 1u << (b - 32);
-    }
+    mark_level(L, pres_lo, pres_hi);
     return L;
 }
 
@@ -358,8 +401,8 @@ __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr
         __syncwarp();
     }
     const double inv = 1.0 / P.resZ;
-    double* posz_g = P.posz + ((int64_t)env * P.R + r) * NPOSE;
-    uint32_t* mask_g = P.maskbits + ((int64_t)env * P.R + r) * 8;
+    double* posz_g = posz_of(P, env, r);
+    uint32_t* mask_g = maskbits_of(P, env, r);
     int lv[8];
     uint32_t pres_lo = 0, pres_hi = 0, any = 0;
     const int Y = lane & 15;
@@ -395,11 +438,7 @@ __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr
         lv[pass] = feasA ? level_of(P, accA, inv, pres_lo, pres_hi, err) : -1;
         lv[pass + 4] = feasB ? level_of(P, accB, inv, pres_lo, pres_hi, err) : -1;
     }
-    pres_lo = __reduce_or_sync(0xffffffffu, pres_lo);
-    pres_hi = __reduce_or_sync(0xffffffffu, pres_hi);
-    const int nl = emit_level_bitmaps(P.bitmaps + ((int64_t)env * P.R + r) * MAX_LEVELS * 8, lane, lv,
-                                      ((uint64_t)pres_hi << 32) | pres_lo);
-    if (lane == 0) P.nlevels[(int64_t)env * P.R + r] = nl;
+    emit_level_bitmaps(P, env, r, lane, lv, pres_lo, pres_hi);
     return any != 0;
 }
 
@@ -429,7 +468,7 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
         __syncwarp();
     }
     const double inv = 1.0 / P.resZ;
-    double* posz_g = P.posz + ((int64_t)env * P.R + r) * NPOSE;
+    double* posz_g = posz_of(P, env, r);
     const uint32_t magic = 65536u / (uint32_t)(nY > 0 ? nY : 1) + 1u;      // v / nY == (v * magic) >> 16 for v < 256, nY <= 16
     // PPL poses per lane: chunks of 128 poses with four accumulators per lane, then what is left (nX * nY is
     // rarely a multiple of 128) with two or one, so the tail does not cost a full four-pose pass
@@ -481,7 +520,7 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
     }
     __syncwarp();
     // fixed-layout pass: feasibility bits, level presence, bitmaps; poses outside the scanned range keep 1e3 / 0
-    uint32_t* mask_g = P.maskbits + ((int64_t)env * P.R + r) * 8;
+    uint32_t* mask_g = maskbits_of(P, env, r);
     int lv[8];
     uint32_t pres_lo = 0, pres_hi = 0, any = 0;
 #pragma unroll
@@ -494,13 +533,9 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
         any |= mb;
         const int L = code - (LEVEL_OFFSET + 1);
         lv[pass] = code ? L : -1;
-        if (code && L != -1) { const int b = L + LEVEL_OFFSET; if (b < 32) pres_lo |= 1u << b; else pres_hi |= 1u << (b - 32); }
+        if (code) mark_level(L, pres_lo, pres_hi);
     }
-    pres_lo = __reduce_or_sync(0xffffffffu, pres_lo);
-    pres_hi = __reduce_or_sync(0xffffffffu, pres_hi);
-    const int nl = emit_level_bitmaps(P.bitmaps + ((int64_t)env * P.R + r) * MAX_LEVELS * 8, lane, lv,
-                                      ((uint64_t)pres_hi << 32) | pres_lo);
-    if (lane == 0) P.nlevels[(int64_t)env * P.R + r] = nl;
+    emit_level_bitmaps(P, env, r, lane, lv, pres_lo, pres_hi);
     return any != 0;
 }
 
@@ -530,12 +565,9 @@ __device__ __forceinline__ void backoff() { __nanosleep(100); }
 constexpr int READY_POLLS = 1 << 16;       // ~10 ms of polling before the fallback
 
 // ---- scan kernel ------------------------------------------------------------------------------------------
-#ifndef IRBPP_SCAN_MIN_CTAS
-#define IRBPP_SCAN_MIN_CTAS 8
-#endif
 // TRAJ: the item source is trajectory replay (idle bins exist); the other sources run the instantiation without that code
 template <bool TRAJ>
-__global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_kernel(const Params P) {
+__global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(const Params P) {
     __shared__ __align__(128) double hm_s[HX * HY];
     extern __shared__ __align__(16) TileEntry estage[];  // CTA_WARPS x P.maxwh: scan list of each warp's rotation
     __shared__ __align__(16) EnvState st_s;              // this bin's scalar state (loaded / stored by warp 0)
@@ -559,14 +591,8 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         if (P.ready && tid == 0) ready_publish(P.ready + vb, P.epoch);      // nothing to hand over, nobody shall wait
         return;
     }
-    long long t_prev = P.phase_cycles ? clock64() : 0;
-    auto phase_mark = [&](int idx) {
-        if (P.phase_cycles && tid == 0) {
-            const long long now = clock64();
-            atomicAdd(P.phase_cycles + idx, (unsigned long long)(now - t_prev));
-            t_prev = now;
-        }
-    };
+    __shared__ long long t_phase;
+    PhaseClock clock(P, t_phase);
 
     // ---- load heightmap (column-parity planes, 8 KB), candidate table and the bin's scalar state ----
     // All of these are first-touch DRAM reads (the agent's forward pass sits between two steps).  The 8 KB
@@ -608,7 +634,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         tb_pf = P.traj_off[st_s.traj_next]; te_pf = P.traj_off[st_s.traj_next + 1];
     }
     if (mode == MODE_STEP && !idle_in) {
-        // while the bulk copies land: the table headers of the item to be placed, all rotations (48 bytes each), so
+        // while the bulk copies land: the table headers of the item to be placed, all rotations (56 bytes each), so
         // that decoding the action does not start another round trip to L2
         static_assert(sizeof(ShapeRot) % 8 == 0, "headers are copied as 8-byte words");
         constexpr int HW = (int)(sizeof(ShapeRot) / 8);
@@ -630,7 +656,6 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         double2* dst = reinterpret_cast<double2*>(hm_g);
         for (int i = tid; i < HX * HY / 2; i += CTA_THREADS) dst[i] = make_double2(0.0, 0.0);
     };
-    bool st_dirty = false;
 
     // ---- phase A: bookkeeping / apply action ----
     if (idle_in) {
@@ -652,7 +677,6 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
             item_sh = live ? queue_g[0] : -1;
         }
         zero_hm_global();
-        st_dirty = true;
         __syncthreads();
     } else if (mode == MODE_STEP) {
         // every thread decodes the action: the whole CTA then fetches the placed rotation's top table (what the
@@ -743,7 +767,6 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
             if (draw_err) err_sh = draw_err;
             item_sh = live ? queue_g[0] : -1;
         }
-        st_dirty = true;
         __syncthreads();
     } else if (mode == MODE_CANDIDATES) {
         if (tid == 0) {
@@ -752,7 +775,6 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
             st_s.order_act = (int)oa;
             item_sh = queue_g[oa];
         }
-        st_dirty = true;
         __syncthreads();
     } else if (mode == MODE_ALL_OBS) {
         if (tid == 0) item_sh = queue_g[slot];
@@ -761,50 +783,25 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         if (tid == 0) item_sh = P.dbg_items[env];
         __syncthreads();
     }
-    phase_mark(0);   // load + phase A
+    clock.mark(0);   // load + phase A
 
     const bool emit_loc = mode_emits_loc(mode, P.K);
     float* obs_g = P.obs + (int64_t)env * P.obs_stride + slot * P.loc_len;
     const int item = item_sh;
     const int ncand = P.sel * 5;
+    const bool idle = TRAJ && item < 0;          // no trajectory left
+    const bool scanned = emit_loc && !idle;      // phase B runs: the observation carries candidate rows
 
-    if (TRAJ && item < 0) {
-        // no trajectory left: an all-zero observation row (no valid candidate); the candidates kernel skips the bin
-        const int width = emit_loc ? P.loc_len : P.order_len;
-        for (int i = tid; i < width; i += CTA_THREADS) obs_g[i] = 0.0f;
-        if (tid == 0) {
-            if (mode != MODE_ALL_OBS) store_error(P, env, err_sh);
-            st_s.next_seq = next_seq;
-        }
-        __syncthreads();
-        if (st_dirty && warp == 0) reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st_s)[lane];
-        if (P.ready) {
-            __syncthreads();
-            if (tid == 0) ready_publish(P.ready + vb, P.epoch);
-        }
-        return;
-    }
+    // the heightmap is final for this call: float32 copy into the observation
+    auto heightmap_to_obs = [&](int off) {
+        for (int i = tid; i < HX * HY; i += CTA_THREADS) obs_g[off + i] = (float)hm_s[hm_index(i >> 5, i & 31)];
+    };
+    if (scanned) {
+        // location observation: [candidate rows | next_item_vec | heightmap], the rows by the candidates kernel
+        heightmap_to_obs(ncand + 9);
+        if (tid < 9) obs_g[ncand + tid] = (tid == 0) ? (float)item : 0.0f;      // next_item_vec (binPhy.py:191)
 
-    // the heightmap is final for this call: float32 copy into the observation, state write-back
-    {
-        const int hm_obs_off = emit_loc ? ncand + 9 : P.K;
-        for (int i = tid; i < HX * HY; i += CTA_THREADS)
-            obs_g[hm_obs_off + i] = (float)hm_s[hm_index(i >> 5, i & 31)];
-    }
-    if (!emit_loc) {
-        // order observation: [next k item ids | heightmap]  (binPhy.py:229-230)
-        for (int i = tid; i < P.K; i += CTA_THREADS) obs_g[i] = (float)queue_g[i];
-        if (tid == 0) { store_error(P, env, err_sh); st_s.next_seq = next_seq; }
-        if (st_dirty && warp == 0) {
-            __syncwarp();
-            reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st_s)[lane];
-        }
-        return;
-    }
-    if (tid < 9) obs_g[ncand + tid] = (tid == 0) ? (float)item : 0.0f;      // next_item_vec (binPhy.py:191)
-
-    // ---- phase B ----
-    {
+        // ---- phase B ----
         int err = 0;
         bool any = false;
         const int tile = P.srot[(int64_t)item * P.R].tile;      // same for every rotation of a shape
@@ -841,23 +838,33 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         if (lane == 0 && any) any_sh = 1;
         if (__any_sync(0xffffffffu, err) && lane == 0) err_sh = 4;
     }
+
+    // calls that do not scan write their rows here: written before phase B they make the trajectory-mode kernel spill
+    if (idle) {
+        // an all-zero observation row (no valid candidate); the candidates kernel skips the bin
+        const int width = emit_loc ? P.loc_len : P.order_len;
+        for (int i = tid; i < width; i += CTA_THREADS) obs_g[i] = 0.0f;
+    } else if (!emit_loc) {
+        // order observation: [next k item ids | heightmap]  (binPhy.py:229-230)
+        heightmap_to_obs(P.K);
+        for (int i = tid; i < P.K; i += CTA_THREADS) obs_g[i] = (float)queue_g[i];
+    }
+
+    // ---- the one exit: error code, state write-back, hand-over flag ----
+    // (phase A changes the state only in calls that own it, so `owns` is also the write-back condition)
+    const bool owns = mode_writes_state(mode, slot, P.K);
     __syncthreads();
     if (tid == 0) {
         // (several CTAs per bin in MODE_ALL_OBS: only error codes are written; the candidates kernel may overwrite
         // with its own code)
         if (mode != MODE_ALL_OBS || err_sh) store_error(P, env, err_sh);
-        const bool write_state = (mode == MODE_STEP || mode == MODE_RESET || mode == MODE_CANDIDATES ||
-                                  (mode == MODE_ALL_OBS && slot == P.K - 1));
-        if (write_state) { st_s.cur_item = item; st_s.mask_any = any_sh; }
+        // cur_item and mask_any describe the scan just made: a call that did not scan leaves them
+        if (scanned && owns) { st_s.cur_item = item; st_s.mask_any = any_sh; }
         st_s.next_seq = next_seq;
     }
-    {
-        const bool write_state = (mode == MODE_STEP || mode == MODE_RESET || mode == MODE_CANDIDATES ||
-                                  (mode == MODE_ALL_OBS && slot == P.K - 1));
-        if (st_dirty || write_state) {
-            __syncthreads();
-            if (warp == 0) reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st_s)[lane];
-        }
+    if (owns) {
+        __syncthreads();
+        if (warp == 0) reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st_s)[lane];
     }
     if (P.ready) {
         // hand-over: all writes of the CTA (scratch, observation, state) happen-before thread 0's release store through
@@ -866,7 +873,7 @@ __global__ void __launch_bounds__(CTA_THREADS, IRBPP_SCAN_MIN_CTAS) irbpp_scan_k
         __syncthreads();
         if (tid == 0) ready_publish(P.ready + vb, P.epoch);
     }
-    phase_mark(1);   // observation heightmap, write-back, scan, level bitmaps
+    clock.mark(1);   // observation heightmap, write-back, scan, level bitmaps
 }
 
 
@@ -880,8 +887,8 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_levels_kernel(const Params 
     __syncthreads();
     int err = 0;
     for (int r = warp; r < P.R; r += CTA_WARPS) {
-        const double* posz_g = P.posz + ((int64_t)env * P.R + r) * NPOSE;
-        const uint32_t* mask_g = P.maskbits + ((int64_t)env * P.R + r) * 8;
+        const double* posz_g = posz_of(P, env, r);
+        const uint32_t* mask_g = maskbits_of(P, env, r);
         int lv[8];
         uint32_t pres_lo = 0, pres_hi = 0;
 #pragma unroll
@@ -889,11 +896,7 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_levels_kernel(const Params 
             const bool feas = (mask_g[pass] >> lane) & 1u;
             lv[pass] = feas ? level_of(P, posz_g[pass * 32 + lane], inv, pres_lo, pres_hi, err) : -1;
         }
-        pres_lo = __reduce_or_sync(0xffffffffu, pres_lo);
-        pres_hi = __reduce_or_sync(0xffffffffu, pres_hi);
-        const int nl = emit_level_bitmaps(P.bitmaps + ((int64_t)env * P.R + r) * MAX_LEVELS * 8, lane, lv,
-                                          ((uint64_t)pres_hi << 32) | pres_lo);
-        if (lane == 0) P.nlevels[(int64_t)env * P.R + r] = nl;
+        emit_level_bitmaps(P, env, r, lane, lv, pres_lo, pres_hi);
     }
     if (err) err_sh = 4;
     __syncthreads();
@@ -932,11 +935,11 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
     int beste = 0x7fffffff;
     for (int e = tid; e < P.R * NPOSE; e += CTA_THREADS) {
         const int r = e >> 8, p = e & 255;
-        const bool feas = (P.maskbits[((int64_t)env * P.R + r) * 8 + (p >> 5)] >> (p & 31)) & 1u;
+        const bool feas = (maskbits_of(P, env, r)[p >> 5] >> (p & 31)) & 1u;
         double s = HEUR_INVALID;
         if (feas) {
             const ShapeRot* sr = P.srot + (int64_t)item * P.R + r;
-            const double z = P.posz[((int64_t)env * P.R + r) * NPOSE + p];
+            const double z = posz_of(P, env, r)[p];
             s = heuristic_score(method, P.heur_dir, p >> 4, p & 15, z, P.resA, AX, AY, STEP, hm_at,
                                 P.Ts + sr->off, sr->w, sr->h);
         }
@@ -1020,9 +1023,9 @@ __host__ __device__ constexpr int cand_smem_bytes(int R) {
 template <int EPC>
 __host__ __device__ constexpr int cand_min_ctas() { return 32 / EPC; }
 constexpr int SM90_SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;
-static_assert(cand_min_ctas<ENVS_PER_CTA_NARROW>() * (cand_smem_bytes<ENVS_PER_CTA_NARROW>(IRBPP_WIDE_MIN_R - 1) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
+static_assert(cand_min_ctas<ENVS_PER_CTA_NARROW>() * (cand_smem_bytes<ENVS_PER_CTA_NARROW>(WIDE_MIN_R - 1) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
               "narrow candidates CTAs at their largest rotation count must fit 32 warps per SM");
-static_assert(cand_min_ctas<ENVS_PER_CTA_WIDE>() * (cand_smem_bytes<ENVS_PER_CTA_WIDE>(IRBPP_WIDE_MIN_R) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
+static_assert(cand_min_ctas<ENVS_PER_CTA_WIDE>() * (cand_smem_bytes<ENVS_PER_CTA_WIDE>(WIDE_MIN_R) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
               "wide candidates CTAs at their smallest rotation count must fit 32 warps per SM");
 
 template <int EPC, bool TRAJ>      // TRAJ: as in irbpp_scan_kernel
@@ -1048,27 +1051,8 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
     }
     const int R = P.R;
     const int npairs = nenv * R;
-    long long t_prev = P.phase_cycles ? clock64() : 0;
-    auto phase_mark = [&](int idx) {
-        if (P.phase_cycles && tid == 0) {
-            const long long now = clock64();
-            atomicAdd(P.phase_cycles + idx, (unsigned long long)(now - t_prev));
-            t_prev = now;
-        }
-    };
-#ifdef IRBPP_PROBE_TRACE
-    // profiling build only: per-CTA timeline (globaltimer, ns) in P.phase_cycles[8 + blockIdx.x * 8 + slot]
-    auto trace = [&](int slot, unsigned long long v = ~0ull) {
-        if (P.phase_cycles && tid == 0) {
-            unsigned long long t;
-            asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-            P.phase_cycles[8 + (size_t)blockIdx.x * 8 + slot] = (v == ~0ull) ? t : v;
-        }
-    };
-    trace(0);
-#else
-    auto trace = [&](int, unsigned long long = 0ull) {};
-#endif
+    long long t_phase;
+    PhaseClock clock(P, t_phase);
     // the "bins" of this kernel are (bin, buffer slot) pairs in MODE_ALL_OBS (see the scan kernel): real bin, slot and
     // the place of a pair's rows in the observation
     const bool all_obs = (P.mode == MODE_ALL_OBS);
@@ -1102,10 +1086,8 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         for (int b = 0; b < npairs; b += 32) {
             const int q = b + lane;
             int c = 0;
-            if (q < npairs && env_live(env0 + q / R)) c = P.nlevels[(int64_t)env0 * R + q];
-            int incl = c;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int tt = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += tt; }
+            if (q < npairs && env_live(env0 + q / R)) c = *(nlevels_of(P, env0, 0) + q);     // pair q = (bin, rotation) of the CTA
+            const int incl = warp_inclusive_scan(c, lane);
             if (q < npairs) S.pre[q + 1] = carry + incl;
             carry += __shfl_sync(0xffffffffu, incl, 31);
         }
@@ -1113,7 +1095,6 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
     }
     __syncthreads();
     const int nimg = S.pre[npairs];
-    trace(1);
     unsigned char* ws_base = smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15);     // CAND_WARPS blocks of WS_BYTES
     uint8_t* W_pts = ws_base + (size_t)warp * WS_BYTES;
 
@@ -1130,8 +1111,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
             const int t = base + tid;
             int lo = 0, hi = npairs;                        // pre[lo] <= t < pre[hi]
             while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (S.pre[mid] <= t) lo = mid; else hi = mid; }
-            const uint4* src = reinterpret_cast<const uint4*>(
-                P.bitmaps + (((int64_t)env0 * R + lo) * MAX_LEVELS + (t - S.pre[lo])) * 8);
+            const uint4* src = reinterpret_cast<const uint4*>(bitmaps_of(P, env0, 0) + ((int64_t)lo * MAX_LEVELS + (t - S.pre[lo])) * 8);
             const uint4 a = src[0], b = src[1];
             uint32_t* rows = S.slots + tid * ROWS_WORDS;
             S.pair_of[tid] = (uint16_t)lo;
@@ -1153,18 +1133,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
             my_off = atomicAdd(&S.hist[bucket], 1);
         }
         __syncthreads();
-        if (warp == 0) {   // exclusive prefix over the 64 buckets
-            const int h0 = S.hist[lane], h1 = S.hist[32 + lane];
-            int i0 = h0, i1 = h1;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int t0 = __shfl_up_sync(0xffffffffu, i0, o), t1 = __shfl_up_sync(0xffffffffu, i1, o);
-                if (lane >= o) { i0 += t0; i1 += t1; }
-            }
-            const int tot0 = __shfl_sync(0xffffffffu, i0, 31);
-            S.hbase[lane] = i0 - h0;
-            S.hbase[32 + lane] = tot0 + i1 - h1;
-        }
+        if (warp == 0) bucket_prefix64(S.hist, S.hbase, lane);
         __syncthreads();
         // position in cost order -> (slot, count); cand_off[] temporarily holds the counts
         int my_pos = 0;
@@ -1176,10 +1145,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         for (int i = nround + tid; i < CAND_THREADS; i += CAND_THREADS) S.cand_off[i + 1] = 0;
         __syncthreads();
         {   // CTA-wide inclusive prefix of the counts in cost order
-            const int c = S.cand_off[tid + 1];
-            int incl = c;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) { const int tt = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += tt; }
+            const int incl = warp_inclusive_scan(S.cand_off[tid + 1], lane);
             if (lane == 31) S.warp_tot[warp] = incl;
             __syncthreads();
             int wbase = 0;
@@ -1204,12 +1170,8 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
             }
         }
         __syncthreads();
-        if (base == 0) trace(2);
-#ifdef IRBPP_PROBE_FINE
-        phase_mark(4);   // prologue, image loads, cost sort, start-pixel prefix
-#else
+        // work counters: level images, start-pixel tasks, rounds
         if (P.phase_cycles && tid == 0) { atomicAdd(P.phase_cycles + 4, (unsigned long long)nround); atomicAdd(P.phase_cycles + 5, (unsigned long long)ntask); atomicAdd(P.phase_cycles + 6, 1ull); }
-#endif
 
         // 2. micro-tasks: one (image, start pixel) pair each, TASKS_PER_LANE per lane and batch.  The tasks are in cost
         //    order, so task slot 0 of the lanes holds the 32 * EPC most expensive ones (FAST_CAP-point scratch), the other
@@ -1263,10 +1225,6 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
             //     of a warp have similar trip counts and abandoned / hole paths drop out
             if (tid < 64) S.hist[tid] = 0;
             __syncthreads();
-            if (base == 0 && mb == 0) trace(3);
-#ifdef IRBPP_PROBE_FINE
-            phase_mark(5);   // find start pixel + follow (incl. waiting for the slowest warp)
-#endif
             int boff[TPL];
 #pragma unroll
             for (int jt = 0; jt < TPL; ++jt) {
@@ -1275,26 +1233,12 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                 S.q_of[jt * CAND_THREADS + tid] = (uint16_t)(tk[jt] >= 0 ? S.pair_of[tk[jt] >> 8] : 0);
             }
             __syncthreads();
-            if (warp == 0) {   // exclusive prefix over the 64 buckets
-                const int h0 = S.hist[lane], h1 = S.hist[32 + lane];
-                int i0 = h0, i1 = h1;
-#pragma unroll
-                for (int o = 1; o < 32; o <<= 1) {
-                    const int t0 = __shfl_up_sync(0xffffffffu, i0, o), t1 = __shfl_up_sync(0xffffffffu, i1, o);
-                    if (lane >= o) { i0 += t0; i1 += t1; }
-                }
-                const int tot0 = __shfl_sync(0xffffffffu, i0, 31);
-                S.hbase[lane] = i0 - h0;
-                S.hbase[32 + lane] = tot0 + i1 - h1;
-            }
+            if (warp == 0) bucket_prefix64(S.hist, S.hbase, lane);
             __syncthreads();
 #pragma unroll
             for (int jt = 0; jt < TPL; ++jt)
                 S.order2[S.hbase[63 - min(63, npts_j[jt])] + boff[jt]] = (uint16_t)(jt * CAND_THREADS + tid);
             __syncthreads();
-#ifdef IRBPP_PROBE_FINE
-            phase_mark(6);   // length sort
-#endif
             // (c) lane i approximates the contours of rank i, i + CAND_THREADS, ... (points live in their owners' scratch)
 #pragma unroll 1
             for (int jt = 0; jt < TPL; ++jt) {
@@ -1310,10 +1254,6 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                 }
             }
             __syncthreads();           // scratch of every lane is free again
-            if (base == 0 && mb == 0) { trace(4); int mx = 0; for (int i = 0; i < BATCH; ++i) mx = max(mx, (int)S.n_of[i]); trace(7, ((unsigned long long)ntask << 8) | (unsigned long long)mx); }
-#ifdef IRBPP_PROBE_FINE
-            phase_mark(7);   // approxPolyDP + emit
-#endif
             // rare: a contour longer than its slot's buffer; the lanes concerned redo it one at a time with
             // 1024-point buffers laid over the (now idle) scratch of this warp
 #pragma unroll 1
@@ -1323,9 +1263,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                     const int src_lane = __ffs((int)ovf) - 1;
                     ovf &= ovf - 1;
                     if (lane == src_lane) {
-#ifndef IRBPP_PROBE_FINE
                         if (P.phase_cycles) atomicAdd(P.phase_cycles + 7, 1ull);     // overflow redo counter
-#endif
                         FlatScratch<BIG_CAP> bs;
                         bs.b = W_pts;
                         const int slot = tk[jt] >> 8, q = S.pair_of[slot];
@@ -1342,8 +1280,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         __syncthreads();
     }
     __syncthreads();
-    trace(5);
-    phase_mark(2);   // contour tasks
+    clock.mark(2);   // contour tasks
     // the scan grid has long completed; waiting for it formally keeps the stream-order guarantee of a dependent launch
     // (this grid does not complete before its prerequisite) without delaying the start
     if (P.ready && tid == 0) grid_dependency_wait();
@@ -1356,21 +1293,17 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
     // ---- phase D ----
     const int sel = P.sel;
     const uint32_t* cbits = candbits + warp * R * 8;
-    const uint32_t* mask_g = P.maskbits + (int64_t)env * R * 8;
-    const double* posz_g = P.posz + (int64_t)env * R * NPOSE;
+    const uint32_t* mask_g = maskbits_of(P, env, 0);
+    const double* posz_g = posz_of(P, env, 0);
     const int renv = real_env(env);
     float* obs_g = P.obs + obs_offset(env);
-    const bool write_state = (P.mode == MODE_STEP || P.mode == MODE_RESET || P.mode == MODE_CANDIDATES ||
-                              (all_obs && slot_of_e(env) == P.K - 1));
-    uint16_t* cand_g = write_state ? P.cand + (int64_t)renv * P.cand_stride : nullptr;
+    uint16_t* cand_g = mode_writes_state(P.mode, slot_of_e(env), P.K) ? P.cand + (int64_t)renv * P.cand_stride : nullptr;
     double* dbg_cand = P.dbg_cand ? P.dbg_cand + (int64_t)env * sel * 5 : nullptr;
 
     // candidate counts per rotation (lane r), exclusive prefix, total
     int cnt = 0;
     if (lane < R) { for (int qd = 0; qd < 8; ++qd) cnt += __popc(cbits[lane * 8 + qd]); }
-    int incl = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int tt = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += tt; }
+    const int incl = warp_inclusive_scan(cnt, lane);
     const int excl = incl - cnt;
     const int Ktot = __shfl_sync(0xffffffffu, incl, 31);
     uint32_t anym = 0;
@@ -1479,10 +1412,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                     int c[BPL], tot = 0;
 #pragma unroll
                     for (int q = 0; q < BPL; ++q) { c[q] = hist[lane * BPL + q]; tot += c[q]; }
-                    int inc = tot;
-#pragma unroll
-                    for (int o = 1; o < 32; o <<= 1) { const int t0 = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t0; }
-                    int base = inc - tot;
+                    int base = warp_inclusive_scan(tot, lane) - tot;
                     __syncwarp();
 #pragma unroll
                     for (int q = 0; q < BPL; ++q) {
@@ -1532,8 +1462,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         if (dev_err) store_error(P, renv, dev_err);
         if (P.dbg_nhull) P.dbg_nhull[env] = Ktot;
     }
-    if (warp == 0) trace(6);
-    phase_mark(3);   // select / pad, candidate rows of the observation
+    clock.mark(3);   // select / pad, candidate rows of the observation
 }
 
 }  // namespace irbpp

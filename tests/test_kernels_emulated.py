@@ -83,9 +83,12 @@ class EmuEnv(object):
         lib.emu_irbpp_obs_len(self.h, ctypes.byref(o), ctypes.byref(l), ctypes.byref(k))
         self.obs_len, self.loc_len = o.value, l.value
 
-    def reset(self):
-        obs = np.zeros((self.n, self.obs_len), np.float32)
-        assert self.lib.emu_irbpp_reset(self.h, None, ctypes.c_void_p(obs.ctypes.data), None) == 0
+    def reset(self, which=None, obs=None):
+        """``which``: reset only the bins where it is nonzero; the other rows of ``obs`` stay as they are."""
+        obs = np.zeros((self.n, self.obs_len), np.float32) if obs is None else obs
+        which_u8 = None if which is None else np.ascontiguousarray(which, dtype=np.uint8)
+        sel = None if which_u8 is None else ctypes.c_void_p(which_u8.ctypes.data)
+        assert self.lib.emu_irbpp_reset(self.h, sel, ctypes.c_void_p(obs.ctypes.data), None) == 0
         return obs
 
     def step_results(self, actions, on_device=0):
@@ -165,6 +168,39 @@ def test_emulated_host_and_device_result_blocks_agree(emu):
         env.close()
 
 
+def test_emulated_partial_reset_and_sequence_wrap(emu):
+    """irbpp_reset with `which`: the scan CTAs of unselected bins return at once and the candidates kernel skips them.
+    The reset rows match fresh oracle episodes, the other rows are untouched, and the steps after it (through the
+    wrap-around of the short sequences) match the oracle."""
+    from irbpp_b200 import shapes
+    from oracle.oracle_env import OracleConfig, OracleEnv
+    lib = shapes.make_blockout_library(8, seed=2)
+    n = 4
+    seqs = shapes.make_sequences(n, 5, lib.num_shapes, seed=9)        # short: the cursor wraps
+    env = EmuEnv(emu, lib, seqs)
+    oracles = [OracleEnv(OracleConfig(ZRotNum=4), lib, seqs[i]) for i in range(n)]
+    obs = env.reset()
+    want = np.stack([o.reset() for o in oracles])
+    assert np.array_equal(obs, want.astype(np.float32))
+    acts = np.array([int(np.argmax(want[i][:2500].reshape(500, 5)[:, 4] == 1)) for i in range(n)])
+    outs = [oracles[i].step(int(acts[i])) for i in range(n)]
+    want = np.stack([o[0] if not o[2] else oracles[i].reset() for i, o in enumerate(outs)])
+    obs = env.step(acts)[0]
+    assert np.array_equal(obs, want.astype(np.float32))
+    before = obs.copy()
+    obs = np.full_like(obs, -7.0)           # neither kernel may write the rows of bins 0 and 2
+    env.reset(np.array([0, 1, 0, 1]), obs)
+    for i in (1, 3):
+        want[i] = oracles[i].reset()
+    assert np.all(obs[[0, 2]] == -7.0)
+    assert np.array_equal(obs[[1, 3]], want[[1, 3]].astype(np.float32))
+    assert np.array_equal(want[[0, 2]].astype(np.float32), before[[0, 2]])
+    for t in range(12):                                              # > 5 draws per bin -> wrap-around
+        acts = np.array([int(np.argmax(want[i][:2500].reshape(500, 5)[:, 4] == 1)) for i in range(n)])
+        outs = [oracles[i].step(int(acts[i])) for i in range(n)]
+        want = np.stack([o[0] if not o[2] else oracles[i].reset() for i, o in enumerate(outs)])
+        assert np.array_equal(env.step(acts)[0], want.astype(np.float32)), t
+    env.close()
 
 
 @pytest.mark.parametrize("sel", [24, 96])

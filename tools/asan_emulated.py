@@ -3,7 +3,7 @@
 access (dynamic shared memory is a heap block of exactly the launch's size, so a wrong size shows up).
 
     LD_PRELOAD=$(gcc -print-file-name=libasan.so) ASAN_OPTIONS=detect_leaks=0 \\
-        python tools/asan_emulated.py [-DIRBPP_TASKS_PER_LANE=2 ...] 2>&1 | grep -E "ERROR|SUMMARY| ok"
+        python tools/asan_emulated.py 2>&1 | grep -E "ERROR|SUMMARY| ok"
 """
 import os
 import sys

@@ -4,7 +4,7 @@
     IRBPP_LIB=irbpp_b200/lib/libirbpp_x.so python tools/kbench.py [--workloads blockout,irregular8,...] [--e2e]
 
 One JSON line per workload: per-step CUDA-event time (L2 flushed between steps, outside the events), the
-torch stand-in policy is NOT inside the events.  Used to compare build variants (tools/variants.py)."""
+torch stand-in policy is NOT inside the events.  Used to compare two builds of the library (IRBPP_LIB)."""
 import argparse
 import json
 import os

@@ -1,10 +1,7 @@
 #!/usr/bin/env python
 """Per-phase SM cycles of the two step kernels on the bench workload (steady state).  GPU only.
 
-    python tools/phase_probe.py                       # default library: phases + work counters
-    IRBPP_LIB=.../libirbpp_fine.so python tools/phase_probe.py
-        # a library built with -DIRBPP_PROBE_FINE (irbpp_b200.build.build(out=..., defs=["-DIRBPP_PROBE_FINE"])):
-        # slots 4-7 then hold cycles of the candidates kernel's sub-phases instead of the work counters
+    python tools/phase_probe.py                       # phases + work counters of the candidates kernel
 
 Thread 0 of every CTA adds clock64() differences to eight counters (include/irbpp.h,
 irbpp_debug_phase_cycles); the numbers are cycles as seen by warp 0 of a CTA, barrier waits included.
@@ -39,17 +36,11 @@ c = env.debug_phase_cycles(False).astype(np.float64) / n
 scan_ctas = N_ENVS
 bins_per_cta = 8 if lib.num_rotations >= 8 else 4          # envs_per_cta_for(R), csrc/irbpp_kernels.cuh
 cand_ctas = N_ENVS // bins_per_cta
-fine = "fine" in os.path.basename(os.environ.get("IRBPP_LIB", ""))
 out = {"lib": os.environ.get("IRBPP_LIB", "default"), "config": CONFIG, "bins_per_candidates_cta": bins_per_cta,
        "scan_kernel_cycles_per_cta": {"load + apply action (phase A)": round(c[0] / scan_ctas),
                                       "observation, pose scan, level bitmaps": round(c[1] / scan_ctas)},
        "candidates_kernel_cycles_per_cta": {"contour tasks (phase C)": round(c[2] / cand_ctas),
-                                            "select / pad (phase D)": round(c[3] / cand_ctas)}}
-if fine:
-    out["candidates_kernel_cycles_per_cta"].update({
-        "C: loads, cost sort, task table": round(c[4] / cand_ctas), "C: find start + follow": round(c[5] / cand_ctas),
-        "C: length sort": round(c[6] / cand_ctas), "C: approxPolyDP + emit": round(c[7] / cand_ctas)})
-else:
-    out["work_per_cta"] = {"level images": round(c[4] / cand_ctas, 1), "start-pixel tasks": round(c[5] / cand_ctas, 1),
-                           "rounds": round(c[6] / cand_ctas, 2), "overflow redos (> 64 points)": round(c[7] / cand_ctas, 3)}
+                                            "select / pad (phase D)": round(c[3] / cand_ctas)},
+       "work_per_cta": {"level images": round(c[4] / cand_ctas, 1), "start-pixel tasks": round(c[5] / cand_ctas, 1),
+                        "rounds": round(c[6] / cand_ctas, 2), "overflow redos (> 64 points)": round(c[7] / cand_ctas, 3)}}
 print(json.dumps(out, indent=1))

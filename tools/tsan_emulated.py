@@ -4,7 +4,7 @@ race check of shared-memory / global hand-overs between the threads of a block (
 the emulator are visible to TSan).  No GPU needed.
 
     LD_PRELOAD=$(gcc -print-file-name=libtsan.so) TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0" \\
-        python tools/tsan_emulated.py episode_irregular [-DIRBPP_TASKS_PER_LANE=2 ...] 2>&1 | grep -E "SUMMARY|replayed"
+        python tools/tsan_emulated.py episode_irregular 2>&1 | grep -E "SUMMARY|replayed"
 
 Known report: irbpp_scan_kernel, `any_sh = 1` written by lane 0 of several warps (same value, idempotent).
 """
