@@ -40,7 +40,8 @@ extern "C" {
 #define IRBPP_ERR_LEVEL     4   /* a drop height quantised outside the level range */
 #define IRBPP_ERR_TRAJ_END  5   /* the bin drew past the end of its trajectory (irbpp_set_trajectories); the
                                  * reference appends None there and fails on it (IRcreator.py:94-101) */
-#define IRBPP_ERR_CONTOUR   6   /* a contour longer than the 1024-point overflow buffer */
+#define IRBPP_ERR_CONTOUR   6   /* a contour longer than the overflow buffer (4 points per pose of the action grid:
+                                 * no contour is that long, so the code is not expected) */
 
 typedef struct irbpp_env* irbpp_handle;
 
@@ -52,7 +53,7 @@ typedef struct irbpp_config {
     int32_t selected_action;   /* --selectedAction, candidate rows per observation (default 500) */
     int32_t buffer_size;       /* --bufferSize k; k > 1 selects the order->location protocol */
     double  bin_dimension[3];  /* [0.32, 0.32, 0.30] (arguments.py:115) */
-    double  resolution_act;    /* --resolutionA 0.02 */
+    double  resolution_act;    /* --resolutionA: 0.02 (16x16 actions) or resolution_h (32x32 actions) */
     double  resolution_h;      /* --resolutionH 0.01 */
     double  resolution_z;      /* --resolutionZ 0.01 (cvTools.py:77 heightResolution) */
     int32_t device;            /* CUDA device ordinal */

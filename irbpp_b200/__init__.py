@@ -6,4 +6,4 @@ in ``include/irbpp.h``), ``vec_env`` (the reference's VecEnv surface on the GPU)
 ``envs`` (``make_vec_envs`` mirror), ``sharding`` (multi-GPU)."""
 __version__ = "0.1.0"
 # Stamp of the CUDA kernels' generation; bench.py only reports ncu DRAM traffic captured for this stamp.
-KERNEL_VERSION = "r03-v28"
+KERNEL_VERSION = "r03-v29"

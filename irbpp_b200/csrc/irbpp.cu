@@ -34,6 +34,8 @@ struct irbpp_env {
     uint32_t* ready_dev = nullptr;       // scan -> candidates hand-over flags (one per unit)
     uint32_t epoch = 0;                  // launch counter behind the flags
     int epc = ENVS_PER_CTA_NARROW;       // bins per CTA of the candidates kernel (envs_per_cta_for(R))
+    int step = 2;                        // stepSize of the action grid (Grid<step>): 2 -> 16x16 actions, 1 -> 32x32
+    int npose = Grid<2>::NPOSE;          // poses per rotation of that grid
     std::string err;
     bool shapes_loaded = false, sequences_set = false, was_reset = false, waiting_step = false;
     bool scan_current = false;        // the scan scratch holds the drop heights of every bin's cur_item
@@ -153,23 +155,34 @@ static void free_dev(irbpp_env* h, void* p) {
     cudaFree(p);
 }
 
-// The step kernels of a configuration: `epc` bins per candidates CTA (envs_per_cta_for(R)), `traj`: the trajectory
-// item source, and the candidates kernel's dynamic shared memory at R rotations.
+// The kernels of a configuration: the action grid (stepSize `step`), `epc` bins per candidates CTA (envs_per_cta_for(R)),
+// `traj`: the trajectory item source, and the candidates kernel's dynamic shared memory at R rotations.
 struct StepKernels {
     void (*scan)(const Params);
     void (*cand)(const Params);
+    void (*levels)(const Params);
+    void (*heur)(const Params);
     int cand_smem;
 };
 
-template <int EPC>
+template <int EPC, class G>
 static StepKernels step_kernels_epc(bool traj, int R) {
-    return {traj ? irbpp_scan_kernel<true> : irbpp_scan_kernel<false>,
-            traj ? irbpp_candidates_kernel<EPC, true> : irbpp_candidates_kernel<EPC, false>, cand_smem_bytes<EPC>(R)};
+    return {traj ? irbpp_scan_kernel<G, true> : irbpp_scan_kernel<G, false>,
+            traj ? irbpp_candidates_kernel<EPC, G, true> : irbpp_candidates_kernel<EPC, G, false>,
+            irbpp_levels_kernel<G>, irbpp_heuristic_kernel<G>, cand_smem_bytes<EPC, G>(R)};
 }
 
-static StepKernels step_kernels(int epc, bool traj, int R) {
-    return epc == ENVS_PER_CTA_WIDE ? step_kernels_epc<ENVS_PER_CTA_WIDE>(traj, R) : step_kernels_epc<ENVS_PER_CTA_NARROW>(traj, R);
+template <class G>
+static StepKernels step_kernels_grid(int epc, bool traj, int R) {
+    return epc == ENVS_PER_CTA_WIDE ? step_kernels_epc<ENVS_PER_CTA_WIDE, G>(traj, R) : step_kernels_epc<ENVS_PER_CTA_NARROW, G>(traj, R);
 }
+
+static StepKernels step_kernels(int step, int epc, bool traj, int R) {
+    return step == 1 ? step_kernels_grid<Grid<1>>(epc, traj, R) : step_kernels_grid<Grid<2>>(epc, traj, R);
+}
+
+// scratch sizes of the grid of stepSize `step`
+static int grid_list_cap_ws(int step) { return step == 1 ? CandScratch<Grid<1>>::LIST_CAP_WS : CandScratch<Grid<2>>::LIST_CAP_WS; }
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-function, PER-DEVICE attribute: the largest value any
 // handle needed is tracked per (device, kernel) and only ever raised (several handles may coexist on a device,
@@ -201,16 +214,21 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
         return fail(nullptr, IRBPP_EINVAL, "buffer_size must be in [1, %d]", MAX_QUEUE);
     if (cfg->selected_action < 1 || cfg->selected_action > 4096)
         return fail(nullptr, IRBPP_EINVAL, "selected_action must be in [1, 4096]");
-    // grid sizes exactly as Space.__init__ computes them (space.py:19-24)
+    // grid sizes exactly as Space.__init__ computes them (space.py:19-24); supported: the 32x32 heightmap with step 2
+    // (16x16 actions) or step 1 (32x32 actions)
     const double stepf = cfg->resolution_act / cfg->resolution_h;
     const int step = (int)stepf;
     const int hx = (int)ceil(cfg->bin_dimension[0] / cfg->resolution_h), hy = (int)ceil(cfg->bin_dimension[1] / cfg->resolution_h);
     const int ax = (int)ceil(cfg->bin_dimension[0] / cfg->resolution_act), ay = (int)ceil(cfg->bin_dimension[1] / cfg->resolution_act);
-    if ((double)step != stepf || step != STEP || hx != HX || hy != HY || ax != AX || ay != AY)
+    const bool grid2 = step == Grid<2>::STEP && ax == Grid<2>::AX && ay == Grid<2>::AY;
+    const bool grid1 = step == Grid<1>::STEP && ax == Grid<1>::AX && ay == Grid<1>::AY;
+    if ((double)step != stepf || hx != HX || hy != HY || !(grid2 || grid1))
         return fail(nullptr, IRBPP_EINVAL,
-                    "unsupported grid: heightmap %dx%d, actions %dx%d, step %g (this build: %dx%d, %dx%d, %d)",
-                    hx, hy, ax, ay, stepf, HX, HY, AX, AY, STEP);
-    if (cfg->selected_action > cfg->num_rotations * NPOSE)
+                    "unsupported grid: heightmap %dx%d, actions %dx%d, step %g (supported: heightmap %dx%d with actions %dx%d, "
+                    "step %d, or actions %dx%d, step %d)",
+                    hx, hy, ax, ay, stepf, HX, HY, Grid<2>::AX, Grid<2>::AY, Grid<2>::STEP, Grid<1>::AX, Grid<1>::AY, Grid<1>::STEP);
+    const int npose = ax * ay;
+    if (cfg->selected_action > cfg->num_rotations * npose)
         return fail(nullptr, IRBPP_EINVAL, "selected_action exceeds the number of poses (reference fallback "
                                            "binPhy.py:217-225 would return a short table)");
     if (!(cfg->resolution_z > 0) || ceil(cfg->bin_dimension[2] / cfg->resolution_z) + 1 >= LEVEL_OFFSET)
@@ -243,6 +261,8 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     P.resA = cfg->resolution_act;
     P.binvol = (cfg->bin_dimension[0] * cfg->bin_dimension[1]) * cfg->bin_dimension[2];   // np.prod
     h->epc = envs_per_cta_for(P.R);                  // bins (= warps) per CTA of the candidates kernel
+    h->step = step; h->npose = npose;
+    const int bmw = npose / 32;
 
 #define TRY_ALLOC(expr)                                                                          \
     do { cudaError_t e2_ = (expr); if (e2_ != cudaSuccess) {                                      \
@@ -255,11 +275,19 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     // scan -> candidates hand-over scratch
     // (buffered: one slice per (bin, buffer slot) pair, get_all_possible_observation scans all of them at once)
     const size_t units = (size_t)N * (size_t)P.K;
-    TRY_ALLOC(dev_alloc(h, &P.posz, units * P.R * NPOSE));
-    TRY_ALLOC(dev_alloc(h, &P.maskbits, units * P.R * 8));
-    TRY_ALLOC(dev_alloc(h, &P.bitmaps, units * P.R * MAX_LEVELS * 8));
+    TRY_ALLOC(dev_alloc(h, &P.posz, units * P.R * npose));
+    TRY_ALLOC(dev_alloc(h, &P.maskbits, units * P.R * bmw));
+    TRY_ALLOC(dev_alloc(h, &P.bitmaps, units * P.R * MAX_LEVELS * bmw));
     TRY_ALLOC(dev_alloc(h, &P.nlevels, units * P.R));
-    if (P.R * NPOSE > LIST_CAP_WS) TRY_ALLOC(dev_alloc(h, &P.dlist, units * 2 * P.R * NPOSE));     // phase-D lists of bins that spill
+    if (P.R * npose > grid_list_cap_ws(step)) TRY_ALLOC(dev_alloc(h, &P.dlist, units * 2 * P.R * npose));     // phase-D lists of bins that spill
+    if (step == 1) {
+        // contour overflow buffers, one per warp of every candidates CTA (a warp redoes one contour at a time).  Every warp
+        // of a CTA takes contour tasks in phase C, the idle warps of a partial last CTA included, so the count is the
+        // units rounded up to whole CTAs
+        static_assert(CandScratch<Grid<1>>::OVF_GLOBAL, "32x32 grid: the overflow buffer lives in global memory");
+        const size_t warps = (units + h->epc - 1) / h->epc * h->epc;
+        TRY_ALLOC(dev_alloc(h, &P.ovf, warps * CandScratch<Grid<1>>::OVF_BYTES, false));
+    }
     TRY_ALLOC(dev_alloc(h, &h->ready_dev, units));        // zeroed: no launch has epoch 0
     const size_t res_bytes = step_results_bytes(N) + 64;
     TRY_ALLOC(cudaMalloc(&h->results_dev, res_bytes));
@@ -272,7 +300,7 @@ int irbpp_create(const irbpp_config* cfg, irbpp_handle* out) {
     TRY_ALLOC(cudaHostAlloc((void**)&h->actions_pinned, 2 * (size_t)N * sizeof(int64_t), cudaHostAllocMapped));
     P.res = step_results(h->results_dev, N);
     for (bool traj : {false, true}) {
-        const StepKernels k = step_kernels(h->epc, traj, P.R);
+        const StepKernels k = step_kernels(step, h->epc, traj, P.R);
         TRY_ALLOC(raise_dynamic_smem(cfg->device, (const void*)k.cand, k.cand_smem));
     }
 #undef TRY_ALLOC
@@ -311,6 +339,7 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
     std::vector<TileEntry> tiles;
     std::vector<double> rew(S);
     int max_entries = 1;
+    const int step = h->step, ax = HX / step, ay = HY / step;
     for (int s = 0; s < S; ++s) {
         rew[s] = (vol[s] / h->P.binvol) * 10;                        // binPhy.py:155-156,321-322
         for (int r = 0; r < R; ++r) {
@@ -320,7 +349,7 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
             if (w <= 0 || hh <= 0 || w > HX || hh > HY || wA <= 0 || hA <= 0)
                 return fail(h, IRBPP_EINVAL, "shape %d rot %d: bad window %dx%d / %dx%d", s, r, w, hh, wA, hA);
             // the reference's window slice would run off the heightmap (NumPy broadcast error, space.py:118)
-            if (w > STEP * wA || hh > STEP * hA)
+            if (w > step * wA || hh > step * hA)
                 return fail(h, IRBPP_EINVAL, "shape %d rot %d: window %dx%d exceeds action footprint %dx%d "
                             "(the reference fails on this table)", s, r, w, hh, wA, hA);
             const int64_t off = offsets[(size_t)s * R + r];
@@ -328,16 +357,16 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
             if (off < 0 || off + 4 * n > maps_len) return fail(h, IRBPP_EINVAL, "shape %d rot %d: table out of range", s, r);
             ShapeRot& q = srot[(size_t)s * R + r];
             q.w = w; q.h = hh;
-            q.nX = AX - wA + 1; q.nY = AY - hA + 1;                  // range(rangeX_A - rangeX_OA + 1)
+            q.nX = ax - wA + 1; q.nY = ay - hA + 1;                  // range(rangeX_A - rangeX_OA + 1)
             if (q.nX < 0) q.nX = 0; if (q.nY < 0) q.nY = 0;
             q.ez = np_round6(e[2]);
             // prejudge (binPhy.py:236,240-241): round(round(l*resA, 6) + extent - bin, 6) > 0 fails
             q.okx = 0; q.oky = 0;
-            for (int l = 0; l < AX; ++l) {
+            for (int l = 0; l < ax; ++l) {
                 const double tx = np_round6((double)l * c.resolution_act);
                 if (!(np_round6(tx + e[0] - c.bin_dimension[0]) > 0)) q.okx |= 1u << l;
             }
-            for (int l = 0; l < AY; ++l) {
+            for (int l = 0; l < ay; ++l) {
                 const double ty = np_round6((double)l * c.resolution_act);
                 if (!(np_round6(ty + e[1] - c.bin_dimension[1]) > 0)) q.oky |= 1u << l;
             }
@@ -355,8 +384,9 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
             q.any_zero = any_zero;
             q.tile = 1; q.tile_off = 0; q.ntiles = 0;
         }
-        // block structure of the bottom tables of shape s (all rotations must agree on the block size)
-        for (int t = 4; t >= 2; t >>= 1) {
+        // block structure of the bottom tables of shape s (all rotations must agree on the block size); step 2 only, where
+        // every window starts on an even cell
+        for (int t = 4; t >= 2 && step == 2; t >>= 1) {
             bool ok = true;
             std::vector<std::vector<TileEntry>> found(R);
             for (int r = 0; r < R && ok; ++r) {
@@ -375,7 +405,7 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
                             }
                         if (!any_open) continue;                  // fully masked block contributes nothing
                         if (any_masked || !same || i1 - bi * t != t || j1 - bj * t != t) { ok = false; break; }
-                        TileEntry e; e.off = 8 * ((bi * t / 2) * 16 + (bj * t / 2)); e.pad = 0; e.b = b0;
+                        TileEntry e; e.off = 8 * ((bi * t / 2) * 16 + (bj * t / 2)); e.off_odd = 0; e.b = b0;
                         found[r].push_back(e);
                     }
             }
@@ -389,7 +419,8 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
             }
         }
         if (srot[(size_t)s * R].tile == 1) {
-            // no block structure: one entry per unmasked cell, offset into the column-parity planes
+            // no block structure: one entry per unmasked cell, offset into the column-parity planes from a window origin in an
+            // even row, and (step 1) from one in an odd row
             for (int r = 0; r < R; ++r) {
                 ShapeRot& q = srot[(size_t)s * R + r];
                 const double* Bq = Bs.data() + q.off;
@@ -398,7 +429,8 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
                     for (int j = 0; j < q.h; ++j) {
                         const double b = Bq[(size_t)i * q.h + j];
                         if (std::isinf(b)) continue;
-                        TileEntry e; e.off = 8 * hm_index(i, j); e.pad = 0; e.b = b;
+                        TileEntry e; e.off = 8 * hm_index(i, j); e.b = b;
+                        e.off_odd = step == 1 ? 8 * (hm_index(i, j + 1) - hm_index(0, 1)) : 0;
                         tiles.push_back(e);
                     }
                 q.ntiles = (int32_t)tiles.size() - q.tile_off;
@@ -429,7 +461,7 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
     // per-warp staging lists, then the bin's candidate table row (bulk-copied by the scan kernel)
     h->scan_smem = CTA_WARPS * h->P.maxwh * (int)sizeof(TileEntry) + ((h->P.cand_stride * 2 + 15) & ~15);
     for (bool traj : {false, true})
-        CUDA_TRY(h, raise_dynamic_smem(c.device, (const void*)step_kernels(h->epc, traj, h->P.R).scan, h->scan_smem));
+        CUDA_TRY(h, raise_dynamic_smem(c.device, (const void*)step_kernels(step, h->epc, traj, h->P.R).scan, h->scan_smem));
     h->shapes_loaded = true;
     return IRBPP_OK;
 }
@@ -570,9 +602,11 @@ static int launch(irbpp_env* h, Params& P, cudaStream_t s) {
     P.ready = (cand_follows && P.mode != MODE_DEBUG_HULLS && P.mode != MODE_ALL_OBS) ? h->ready_dev : nullptr;
     if (++h->epoch == 0) h->epoch = 1;
     P.epoch = h->epoch;
-    const StepKernels k = step_kernels(h->epc, P.item_src == ITEMS_TRAJ, P.R);
-    if (P.mode == MODE_DEBUG_HULLS) irbpp_levels_kernel<<<P.N, CTA_THREADS, 0, s>>>(P);
-    else {
+    const StepKernels k = step_kernels(h->step, h->epc, P.item_src == ITEMS_TRAJ, P.R);
+    if (P.mode == MODE_DEBUG_HULLS) {
+        void (*levels)(const Params) = k.levels;
+        levels<<<P.N, CTA_THREADS, 0, s>>>(P);
+    } else {
         void (*scan)(const Params) = k.scan;
         scan<<<units, CTA_THREADS, h->scan_smem, s>>>(P);
     }
@@ -745,7 +779,8 @@ int irbpp_heuristic_actions(irbpp_handle h, int32_t method, int32_t dir_idx, int
     P.heur_method = method; P.heur_dir = dir_idx;
     P.heur_pose = (on_device && poses_out) ? poses_out : h->heur_pose_dev;
     P.heur_index = (on_device && index_out) ? index_out : h->heur_index_dev;
-    irbpp_heuristic_kernel<<<P.N, CTA_THREADS, 0, s>>>(P);
+    void (*heur)(const Params) = step_kernels(h->step, h->epc, false, P.R).heur;
+    heur<<<P.N, CTA_THREADS, 0, s>>>(P);
     h->launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return fail(h, IRBPP_ECUDA, "kernel launch: %s", cudaGetErrorString(e));
@@ -800,7 +835,7 @@ int irbpp_debug_set_heightmap(irbpp_handle h, const double* heightmap) {
 
 static int debug_run(irbpp_env* h, Params& P, double* posZmap, double* posZValid, double* naiveMask,
                      double* cand, int32_t* num_hull) {
-    const size_t N = P.N, nm = N * P.R * NPOSE, nc = N * P.sel * 5;
+    const size_t N = P.N, nm = N * P.R * h->npose, nc = N * P.sel * 5;
     double* d_cd = nullptr; int32_t* d_nh = nullptr; float* d_obs = nullptr;
     auto cleanup = [&]() { cudaFree(d_cd); cudaFree(d_nh); cudaFree(d_obs); };
 #define DBG_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { cleanup(); return fail(h, IRBPP_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); } } while (0)
@@ -812,7 +847,7 @@ static int debug_run(irbpp_env* h, Params& P, double* posZmap, double* posZValid
     DBG_TRY(cudaDeviceSynchronize());
     if (posZmap || posZValid || naiveMask) {       // float64 views straight from the hand-over scratch
         std::vector<double> pz(nm);
-        std::vector<uint32_t> mb(N * P.R * 8);
+        std::vector<uint32_t> mb(nm / 32);
         DBG_TRY(cudaMemcpy(pz.data(), P.posz, nm * 8, cudaMemcpyDeviceToHost));
         DBG_TRY(cudaMemcpy(mb.data(), P.maskbits, mb.size() * 4, cudaMemcpyDeviceToHost));
         for (size_t i = 0; i < nm; ++i) {
@@ -852,8 +887,8 @@ int irbpp_debug_hulls(irbpp_handle h, const double* posZValid, const double* mas
     int rc = ready(h); if (rc) return rc;
     DeviceGuard guard(h->cfg.device);
     if (!posZValid || !mask) return fail(h, IRBPP_EINVAL, "null argument");
-    const size_t nm = (size_t)h->P.N * h->P.R * NPOSE;
-    std::vector<uint32_t> mb((size_t)h->P.N * h->P.R * 8, 0u);
+    const size_t nm = (size_t)h->P.N * h->P.R * h->npose;
+    std::vector<uint32_t> mb(nm / 32, 0u);
     for (size_t i = 0; i < nm; ++i) if (mask[i] != 0.0) mb[i >> 5] |= 1u << (i & 31);
     CUDA_TRY(h, cudaDeviceSynchronize());
     CUDA_TRY(h, cudaMemcpy(h->P.posz, posZValid, nm * 8, cudaMemcpyHostToDevice));

@@ -1,4 +1,4 @@
-// irbpp_contour.cuh -- per-thread candidate extraction on one 16x16 level image.
+// irbpp_contour.cuh -- per-thread candidate extraction on one level image of the action grid (16x16 or 32x32).
 //
 // Device restatement of what the reference obtains from OpenCV at
 //   cvTools.py:86  cv2.findContours(check, RETR_TREE, CHAIN_APPROX_SIMPLE)  + find_out_contour (:7-38)
@@ -6,9 +6,11 @@
 //   cvTools.py:92  find_convex_vetex (:40-59)
 // (paths relative to the reference root).  Algorithms: border following with the outer start rule of
 // Suzuki-Abe and the CHAIN_APPROX_SIMPLE emission rule, one independent task per start pixel (see
-// below); Douglas-Peucker with OpenCV's closed-curve seeding and clean-up pass.  All arithmetic is integer (coordinates are 0..15), so there is nothing to round: the float
-// comparisons OpenCV performs are between exactly representable values and are restated as integer
-// cross-multiplications.
+// below); Douglas-Peucker with OpenCV's closed-curve seeding and clean-up pass.  All arithmetic is integer (coordinates are
+// 0..A-1 with A = 16 or 32), so there is nothing to round: the float comparisons OpenCV performs are between exactly
+// representable values and are restated as integer cross-multiplications.  They stay exact in int32: for coordinates
+// below 32 every coordinate difference is at most 31 in magnitude, so |cross|, |dot| and seg^2 are at most 2 * 31^2 = 1922
+// and the squared measures (cr^2 + t^2, dist^2) at most 2 * 1922^2 < 2^23.
 //
 // The followers read the level image in padded row form (ROWS_WORDS words, see below).  Border
 // following works on the 8-neighbourhood ring of the current pixel (one byte built from three row
@@ -21,6 +23,19 @@
 
 namespace irbpp {
 
+// An A x A level image, A = 1 << LOG: 16 (stepSize 2, the 16x16 action grid) or 32 (stepSize 1).  A contour point is
+// x << LOG | y (one byte at A = 16, two at A = 32).  The padded row form (what the followers read) has ROWS_WORDS words:
+//   A = 16: rows[y + 1] = (row y) << 1 (bit x + 1 = column x), rows[0] = rows[17] = 0, one pad word;
+//   A = 32: rows[y + 1] = row y (bit x = column x), rows[0] = rows[33] = 0, one pad word (odd stride between the images
+//           of neighbouring threads); the guard columns -1 and 32 come from widening a row to 64 bits when it is read.
+template <int LOG_>
+struct ImageGrid {
+    static constexpr int LOG = LOG_, A = 1 << LOG_, MASK = A - 1;
+    using Point = typename std::conditional<(2 * LOG_ <= 8), uint8_t, uint16_t>::type;
+    static constexpr int ROWS_WORDS = A + 3;
+    static_assert(LOG_ == 4 || LOG_ == 5, "level images are 16x16 or 32x32");
+};
+
 // direction codes, image y grows downward: 0=E 1=NE 2=N 3=NW 4=W 5=SW 6=S 7=SE
 __device__ __forceinline__ int ddx(int s) {
     // dx+1 = {2,2,1,0,0,0,1,2} packed 2 bits each, s = 0 in the low bits
@@ -32,14 +47,16 @@ __device__ __forceinline__ int ddy(int s) {
 }
 
 // ---- scratch accessors -------------------------------------------------------------------------
-template <int STRIDE, int CAP_>
+template <int STRIDE, int CAP_, int LOG_ = 4>
 struct StridedScratch {
     static constexpr int CAP = CAP_;
+    using Grid = ImageGrid<LOG_>;
+    using Point = typename Grid::Point;
     static_assert(CAP_ <= 64, "kept-set is one register pair at most");
-    uint8_t* b;    // CAP contour points, element stride STRIDE
+    Point* b;      // CAP contour points, element stride STRIDE
     typename std::conditional<(CAP_ <= 32), uint32_t, uint64_t>::type kept;
     __device__ __forceinline__ int pt(int i) const { return b[i * STRIDE]; }
-    __device__ __forceinline__ void set_pt(int i, int v) { b[i * STRIDE] = (uint8_t)v; }
+    __device__ __forceinline__ void set_pt(int i, int v) { b[i * STRIDE] = (Point)v; }
     __device__ __forceinline__ void kept_clear(int) { kept = 0; }
     __device__ __forceinline__ void kept_set(int i) { kept |= (decltype(kept))1 << i; }
     __device__ __forceinline__ int kept_count(int) const {
@@ -59,24 +76,29 @@ struct StridedScratch {
     }
 };
 
-template <int CAP_>
+template <int CAP_, int LOG_ = 4>
 struct FlatScratch {
     static constexpr int CAP = CAP_;
+    using Grid = ImageGrid<LOG_>;
+    using Point = typename Grid::Point;
+    static constexpr int KEPT = CAP_ * (int)sizeof(Point);       // byte offset of the kept flags
+    static constexpr int BYTES = KEPT + CAP_;
+    static_assert(CAP_ <= 4096, "RangeStack<false> holds 2 + log2(CAP) ranges");
     uint8_t* b;      // CAP points, CAP kept flags
-    __device__ __forceinline__ int pt(int i) const { return b[i]; }
-    __device__ __forceinline__ void set_pt(int i, int v) { b[i] = (uint8_t)v; }
-    __device__ __forceinline__ void kept_clear(int n) { for (int i = 0; i < n; ++i) b[CAP + i] = 0; }
-    __device__ __forceinline__ void kept_set(int i) { b[CAP + i] = 1; }
-    __device__ __forceinline__ int kept_count(int n) const { int c = 0; for (int i = 0; i < n; ++i) c += b[CAP + i]; return c; }
+    __device__ __forceinline__ int pt(int i) const { return reinterpret_cast<const Point*>(b)[i]; }
+    __device__ __forceinline__ void set_pt(int i, int v) { reinterpret_cast<Point*>(b)[i] = (Point)v; }
+    __device__ __forceinline__ void kept_clear(int n) { for (int i = 0; i < n; ++i) b[KEPT + i] = 0; }
+    __device__ __forceinline__ void kept_set(int i) { b[KEPT + i] = 1; }
+    __device__ __forceinline__ int kept_count(int n) const { int c = 0; for (int i = 0; i < n; ++i) c += b[KEPT + i]; return c; }
     __device__ __forceinline__ int kept_next(int i, int n) const {
         int k = i;
-        do { k = (k + 1 == n) ? 0 : k + 1; } while (!b[CAP + k] && k != i);
+        do { k = (k + 1 == n) ? 0 : k + 1; } while (!b[KEPT + k] && k != i);
         return k;
     }
 };
 
 // Explicit stack of the Douglas-Peucker ranges.  The larger half of a split is deferred, so the depth is
-// at most 2 + log2(n).  For <= 64-point contours the entries (two 6-bit indices) live in a 128-bit shift
+// at most 2 + log2(n) (14 for the 4096-point overflow buffers of 32x32 images).  For <= 64-point contours the entries (two 6-bit indices) live in a 128-bit shift
 // register instead of local memory: pushes and pops are on the dependent chain of the recursion.
 template <bool SMALL>
 struct RangeStack;
@@ -111,6 +133,7 @@ struct RangeStack<false> {
 // index `pos`: OpenCV's clean-up pass over the kept ring, then find_convex_vetex (cvTools.py:40-59).
 template <class S, class Emit>
 __device__ void finish_polygon(S& sc, int n, int pos, Emit emit) {
+    constexpr int SH = S::Grid::LOG, MK = S::Grid::MASK;
     // 3. ring Q = kept points in contour order starting at pos; OpenCV's clean-up pass removes nearly
     // collinear points on diagonal chords.  It writes into a copy of Q and returns the first
     // `new_count` entries; that sequence is regenerated on the fly here instead of being stored.
@@ -126,10 +149,10 @@ __device__ void finish_polygon(S& sc, int n, int pos, Emit emit) {
         int i = 0, writes = 0;
         while (i < c && new_count > 2) {
             const int end = sc.pt(ci); ci = sc.kept_next(ci, n);
-            const int dx = (end >> 4) - (start >> 4), dy = (end & 15) - (start & 15);
-            const int px = (pt >> 4) - (start >> 4), py = (pt & 15) - (start & 15);
+            const int dx = (end >> SH) - (start >> SH), dy = (end & MK) - (start & MK);
+            const int px = (pt >> SH) - (start >> SH), py = (pt & MK) - (start & MK);
             int dist = px * dy - py * dx; if (dist < 0) dist = -dist;
-            const int ip = px * ((end >> 4) - (pt >> 4)) + py * ((end & 15) - (pt & 15));
+            const int ip = px * ((end >> SH) - (pt >> SH)) + py * ((end & MK) - (pt & MK));
             if (2 * dist * dist <= dx * dx + dy * dy && dx != 0 && dy != 0 && ip >= 0) {
                 --new_count;
                 start = end;
@@ -156,15 +179,15 @@ __device__ void finish_polygon(S& sc, int n, int pos, Emit emit) {
         // nothing dropped: the polygon is Q itself
         if (c <= 3) {
             int ci = pos;
-            for (int k = 0; k < c; ++k) { const int p = sc.pt(ci); emit(p >> 4, p & 15); ci = sc.kept_next(ci, n); }
+            for (int k = 0; k < c; ++k) { const int p = sc.pt(ci); emit(p >> SH, p & MK); ci = sc.kept_next(ci, n); }
         } else {
             int a = sc.pt(last), ci = pos, bpt = sc.pt(ci);
             for (int k = 0; k < c; ++k) {
                 ci = sc.kept_next(ci, n);
                 const int cpt = sc.pt(ci);
-                const int abx = (bpt >> 4) - (a >> 4), aby = (bpt & 15) - (a & 15);
-                const int acx = (cpt >> 4) - (a >> 4), acy = (cpt & 15) - (a & 15);
-                if (abx * acy - aby * acx < 0) emit(bpt >> 4, bpt & 15);      // find_convex_vetex: cross < 0
+                const int abx = (bpt >> SH) - (a >> SH), aby = (bpt & MK) - (a & MK);
+                const int acx = (cpt >> SH) - (a >> SH), acy = (cpt & MK) - (a & MK);
+                if (abx * acy - aby * acx < 0) emit(bpt >> SH, bpt & MK);      // find_convex_vetex: cross < 0
                 a = bpt; bpt = cpt;
             }
         }
@@ -173,9 +196,9 @@ __device__ void finish_polygon(S& sc, int n, int pos, Emit emit) {
     if (nc <= 3) {
         // result = dst[0..nc): written values first, untouched copies of Q beyond them
         int k = 0;
-        cleanup([&](int v) { emit(v >> 4, v & 15); ++k; }, nc);
+        cleanup([&](int v) { emit(v >> SH, v & MK); ++k; }, nc);
         int ci = pos;
-        for (int q = 0; q < nc; ++q) { if (q >= k) { const int p = sc.pt(ci); emit(p >> 4, p & 15); } ci = sc.kept_next(ci, n); }
+        for (int q = 0; q < nc; ++q) { if (q >= k) { const int p = sc.pt(ci); emit(p >> SH, p & MK); } ci = sc.kept_next(ci, n); }
         (void)writes;
         return;
     }
@@ -183,9 +206,9 @@ __device__ void finish_polygon(S& sc, int n, int pos, Emit emit) {
     {
         int w0 = -1, w1 = -1, a = -1, bpt = -1, k = 0;
         auto test = [&](int A, int B, int C) {
-            const int abx = (B >> 4) - (A >> 4), aby = (B & 15) - (A & 15);
-            const int acx = (C >> 4) - (A >> 4), acy = (C & 15) - (A & 15);
-            if (abx * acy - aby * acx < 0) emit(B >> 4, B & 15);
+            const int abx = (B >> SH) - (A >> SH), aby = (B & MK) - (A & MK);
+            const int acx = (C >> SH) - (A >> SH), acy = (C & MK) - (A & MK);
+            if (abx * acy - aby * acx < 0) emit(B >> SH, B & MK);
         };
         cleanup([&](int v) {
             if (k == 0) { w0 = v; a = v; }
@@ -219,7 +242,7 @@ __device__ __forceinline__ void farthest_on_arc(const S& sc, int n, int s, int l
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int p = sc.pt(kk[j]);
-            const int px = p >> 4, py = p & 15;
+            const int px = p >> S::Grid::LOG, py = p & S::Grid::MASK;
             const int cr = py * dx - px * dy - c0;
             int v;
             if (legacy) v = cr < 0 ? -cr : cr;
@@ -240,8 +263,9 @@ __device__ __forceinline__ void farthest_on_arc(const S& sc, int n, int s, int l
 // Emits the selected vertices through `emit(x, y)`.
 template <class S, class Emit>
 __device__ void approx_and_emit(S& sc, int n, bool legacy, Emit emit) {
-    auto PX = [&](int i) { return sc.pt(i) >> 4; };
-    auto PY = [&](int i) { return sc.pt(i) & 15; };
+    constexpr int SH = S::Grid::LOG, MK = S::Grid::MASK;
+    auto PX = [&](int i) { return sc.pt(i) >> SH; };
+    auto PY = [&](int i) { return sc.pt(i) & MK; };
     if (n == 4) {
         // Filled axis-aligned rectangle with both sides >= 2 (the common level-set component): the
         // border is (x0,y0),(x0,y1),(x1,y1),(x1,y0).  Every corner is at squared distance
@@ -249,9 +273,9 @@ __device__ void approx_and_emit(S& sc, int n, bool legacy, Emit emit) {
         // fails, and all four turns have the same sign, so approxPolyDP + find_convex_vetex return
         // exactly the four corners.
         const int p0 = sc.pt(0), p1 = sc.pt(1), p2 = sc.pt(2), p3 = sc.pt(3);
-        if ((p0 >> 4) == (p1 >> 4) && (p1 & 15) == (p2 & 15) && (p2 >> 4) == (p3 >> 4) && (p3 & 15) == (p0 & 15) &&
-            (p1 & 15) - (p0 & 15) >= 2 && (p2 >> 4) - (p1 >> 4) >= 2) {
-            emit(p0 >> 4, p0 & 15); emit(p1 >> 4, p1 & 15); emit(p2 >> 4, p2 & 15); emit(p3 >> 4, p3 & 15);
+        if ((p0 >> SH) == (p1 >> SH) && (p1 & MK) == (p2 & MK) && (p2 >> SH) == (p3 >> SH) && (p3 & MK) == (p0 & MK) &&
+            (p1 & MK) - (p0 & MK) >= 2 && (p2 >> SH) - (p1 >> SH) >= 2) {
+            emit(p0 >> SH, p0 & MK); emit(p1 >> SH, p1 & MK); emit(p2 >> SH, p2 & MK); emit(p3 >> SH, p3 & MK);
             return;
         }
     }
@@ -261,7 +285,7 @@ __device__ void approx_and_emit(S& sc, int n, bool legacy, Emit emit) {
         pos += far; if (pos >= n) pos -= n;
         const int pp = sc.pt(pos);
         int best, bi;
-        farthest_on_arc(sc, n, pos, n, pp >> 4, pp & 15, 1, 0, 0, false, best, bi);
+        farthest_on_arc(sc, n, pos, n, pp >> SH, pp & MK, 1, 0, 0, false, best, bi);
         maxd = best > 0 ? best : 0;
         far = bi - pos; if (far < 0) far += n;
         if (maxd == 0) far = 0;
@@ -284,8 +308,8 @@ __device__ void approx_and_emit(S& sc, int n, bool legacy, Emit emit) {
             int len = e - s; if (len <= 0) len += n;
             if (len == 1) { sc.kept_set(s); break; }
             const int ps = sc.pt(s), pe = sc.pt(e);
-            const int sx = ps >> 4, sy = ps & 15;
-            int dx = (pe >> 4) - sx, dy = (pe & 15) - sy;
+            const int sx = ps >> SH, sy = ps & MK;
+            int dx = (pe >> SH) - sx, dy = (pe & MK) - sy;
             const int seg2 = dx * dx + dy * dy;
             // Squared distance to the segment times seg2 (4.13 rule).  With cr = v x d and dot = v . d,
             // |v|^2 |d|^2 = cr^2 + dot^2 (Lagrange), and for w = v - d: w x d = cr, w . d = dot - seg2, so
@@ -314,16 +338,19 @@ __device__ void approx_and_emit(S& sc, int n, bool legacy, Emit emit) {
 // component (nested islands included): its outer border, followed from the component's raster-first
 // pixel.  That pixel has background at W, NW, N and NE; every pixel with that local property is a start
 // candidate (bit mask per row below).
-// Padded row form of a level image (what the followers read): ROWS_WORDS words, rows[y + 1] = (row y) << 1
-// (bit x + 1 = column x), rows[0] = rows[17] = 0, one pad word: no bounds tests, no half-word extraction.
-constexpr int ROWS_WORDS = 19;
+// Padded row form of a level image: ImageGrid::ROWS_WORDS words (see ImageGrid), no bounds tests.
+constexpr int ROWS_WORDS = ImageGrid<4>::ROWS_WORDS;
 
-// start-candidate mask of row y from the row and the row above it (16-bit, unshifted)
+// start-candidate mask of row y from the row and the row above it (A-bit rows, unshifted)
+template <int A = 16>
 __device__ __forceinline__ uint32_t start_mask(uint32_t f, uint32_t up) {
-    return f & ~(f << 1) & ~(up | (up << 1) | (up >> 1)) & 0xFFFFu;
+    constexpr uint32_t ROW = A == 32 ? 0xFFFFFFFFu : (1u << A) - 1u;
+    return f & ~(f << 1) & ~(up | (up << 1) | (up >> 1)) & ROW;
 }
+template <int LOG = 4>
 __device__ __forceinline__ uint32_t start_candidates_rows(const uint32_t* rows, int y) {
-    return start_mask(rows[y + 1] >> 1, rows[y] >> 1);
+    if constexpr (LOG == 4) return start_mask(rows[y + 1] >> 1, rows[y] >> 1);
+    else return start_mask<32>(rows[y + 1], rows[y]);
 }
 
 // ---- micro-task formulation -------------------------------------------------------------------------------
@@ -337,18 +364,24 @@ __device__ __forceinline__ uint32_t start_candidates_rows(const uint32_t* rows, 
 // was abandoned (not a raster-first start) -- in which case nothing must be emitted.
 template <class S>
 __device__ int follow_outer_rows(S& sc, const uint32_t* rows, int x0, int y0, int& area2, int cap = S::CAP) {
+    constexpr int SH = S::Grid::LOG;
+    // columns x-1, x, x+1 of padded row word y as bits 0..2
+    auto cols3 = [&](int y, int x) -> uint32_t {
+        if constexpr (SH == 4) return (rows[y] >> x) & 7u;
+        else return (uint32_t)((((uint64_t)rows[y]) << 1) >> x) & 7u;
+    };
     // 8-neighbourhood ring of pixel (x, y), bit d = neighbour in direction d
     auto ring_at = [&](int x, int y) -> uint32_t {
-        const uint32_t wm = (rows[y] >> x) & 7u;        // bit0 = col x-1, bit1 = col x, bit2 = col x+1
-        const uint32_t w0 = (rows[y + 1] >> x) & 7u;
-        const uint32_t wp = (rows[y + 2] >> x) & 7u;
+        const uint32_t wm = cols3(y, x);                 // bit0 = col x-1, bit1 = col x, bit2 = col x+1
+        const uint32_t w0 = cols3(y + 1, x);
+        const uint32_t wp = cols3(y + 2, x);
         const uint32_t lo = (w0 >> 2) | ((wm & 4u) >> 1) | ((wm & 2u) << 1) | ((wm & 1u) << 3);   // E, NE, N, NW
         return lo | ((w0 & 1u) << 4) | (wp << 5);                                                    // W, SW, S, SE
     };
     uint32_t ring = ring_at(x0, y0);
     area2 = 0;
     if (!ring) {  // isolated pixel
-        sc.set_pt(0, (x0 << 4) | y0);
+        sc.set_pt(0, (x0 << SH) | y0);
         return 1;
     }
     int s;
@@ -369,7 +402,7 @@ __device__ int follow_outer_rows(S& sc, const uint32_t* rows, int x0, int y0, in
         if (p4 < p0) return -2;                          // a pixel of this border precedes the start
         a2 += x3 * y4 - x4 * y3;
         if (s != prev_s) {
-            if (n < cap) sc.set_pt(n, (x3 << 4) | y3);
+            if (n < cap) sc.set_pt(n, (x3 << SH) | y3);
             ++n;
         }
         prev_s = s;
@@ -397,8 +430,8 @@ __device__ bool process_start_candidate(S& sc, const uint32_t* rows, int x, int 
 template <class S, class Emit>
 __device__ bool process_level_image_mt(S& sc, const uint32_t* rows, bool legacy, Emit emit) {
     bool ok = true;
-    for (int y = 0; y < 16; ++y) {
-        uint32_t c = start_candidates_rows(rows, y);
+    for (int y = 0; y < S::Grid::A; ++y) {
+        uint32_t c = start_candidates_rows<S::Grid::LOG>(rows, y);
         while (c) {
             const int x = __ffs((int)c) - 1;
             c &= c - 1;

@@ -8,7 +8,7 @@
 //        heightmap + next_item_vec into the observation (binPhy.py:196-203); state write-back
 //     B  scan every (rotation, X, Y) pose for the next item: drop height + feasibility
 //        (space.py:98-129), one warp per rotation, lanes = poses; level quantisation with NumPy
-//        floor_divide semantics (cvTools.py:78-79); one 16x16 bitmap per (rotation, level) by warp
+//        floor_divide semantics (cvTools.py:78-79); one Ax x Ay bitmap per (rotation, level) by warp
 //        ballots -> global scratch (L2 resident).  Tables that are constant on square blocks of cells
 //        (voxel shapes) are scanned from block maxima of the heightmap (TileEntry lists)
 //   irbpp_candidates_kernel  one CTA per 4 bins (up to seven rotations) or 8 bins (from R = 8), one warp per bin
@@ -16,7 +16,7 @@
 //        ordered by a cost key; every (image, start pixel) pair is one lane's task, dealt in that order
 //        so that the lanes of a warp carry contours of similar length: border following, then (after
 //        re-dealing the contours by length) approxPolyDP + convex filter (irbpp_contour.cuh), results
-//        OR-ed into a 256-bit set per (bin, rotation) in shared memory (np.unique == sorted set)
+//        OR-ed into an Ax*Ay-bit set per (bin, rotation) in shared memory (np.unique == sorted set)
 //     D  select / pad (binPhy.py:205-225): one warp per bin ranks the set bits and writes the
 //        candidate rows of the observation (float32, envs.py:151,163 cast) and the packed candidate
 //        table the next step decodes its action from
@@ -30,6 +30,10 @@
 //
 // Arithmetic is IEEE float64 exactly as NumPy performs it (compile with -fmad=false); masks are
 // folded into the tables as +/-inf sentinels at load time, which changes no comparison result.
+//
+// Every kernel is instantiated per action grid (Grid<STEP>): stepSize 2 (16x16 actions, the reference's default
+// resolutionA = 0.02) and stepSize 1 (32x32 actions, resolutionA = resolutionH = 0.01, what the reference trains the
+// Cube dataset with).  Both use the 32x32 heightmap.
 #pragma once
 #include <stdint.h>
 #include <math.h>
@@ -41,9 +45,22 @@
 namespace irbpp {
 
 constexpr int HX = 32, HY = 32;          // heightmap cells (rangeX_C, rangeY_C)
-constexpr int AX = 16, AY = 16;          // action grid (rangeX_A, rangeY_A)
-constexpr int STEP = 2;                  // stepSize = resolutionAct / resolutionH
-constexpr int NPOSE = AX * AY;           // 256 poses per rotation
+
+// The action grid of stepSize = resolutionAct / resolutionH (space.py:19-24): 2 -> 16x16 actions, 1 -> 32x32.  A pose
+// (rot, lx, ly) is the flat index (rot * AX + lx) * AY + ly == rot << 2 LOG | lx << LOG | ly, which is also the packed
+// form of the candidate table (15 bits at most: rot < 32, LOG <= 5, so it fits uint16).
+template <int STEP_>
+struct Grid {
+    static constexpr int STEP = STEP_;
+    static constexpr int AX = HX / STEP_, AY = HY / STEP_;     // rangeX_A, rangeY_A
+    static constexpr int LOG = STEP_ == 2 ? 4 : 5;             // log2(AY)
+    static constexpr int MASK = AY - 1;
+    static constexpr int NPOSE = AX * AY;                      // 256 / 1024 poses per rotation
+    static constexpr int BMW = NPOSE / 32;                     // words of a pose bit set (feasibility, level image, candidates)
+    using Img = ImageGrid<LOG>;
+    static_assert((STEP_ == 1 || STEP_ == 2) && AX == AY && AY == (1 << LOG), "supported action grids: 16x16 and 32x32");
+    __host__ __device__ static int pack(int rot, int x, int y) { return (rot << (2 * LOG)) | (x << LOG) | y; }
+};
 constexpr int CTA_THREADS = 128;
 constexpr int CTA_WARPS = CTA_THREADS / 32;
 // CTA shapes of the candidates kernel (one warp per bin): 4 bins per CTA below WIDE_MIN_R rotations, 8 from there on.  Both are
@@ -57,9 +74,9 @@ __host__ __device__ inline int envs_per_cta_for(int R) { return R >= WIDE_MIN_R 
 constexpr int MAX_LEVELS = 64;           // level-image slots per (bin, rotation) in the scratch
 constexpr int TASKS_PER_LANE = 2;        // micro-tasks a lane takes per batch of the candidates kernel (one follow / sort / approximate cycle)
 constexpr int SCAN_MIN_CTAS = 8;         // scan CTAs per SM the scan kernel is built for (64 registers per thread)
+constexpr int SCAN_MIN_CTAS_FINE = 6;    // the same on the 32x32 grid (80 registers: with 64 the dense scan's 32 poses per lane spill)
 constexpr int TASK_TAB = 384;            // start pixels of a round listed explicitly (the rest are found by search)
 constexpr int FAST_CAP = 64;             // contour points on the fast path (32 was measured slower: every overflow redo stalls a warp)
-constexpr int BIG_CAP = 1024;            // contour points on the overflow path
 constexpr int LEVEL_OFFSET = 32;         // levels in [-32, 31] -> presence bit (level + 32)
 constexpr int MAX_QUEUE = 16;            // buffer_size limit
 constexpr int MAX_ROT = 32;
@@ -79,7 +96,8 @@ struct ShapeRot {          // one (shape, rotation) entry, device resident
     int32_t nX, nY;        // number of X / Y positions scanned: A - ceil(ext/resA) + 1 (space.py:115-116)
     uint32_t okx, oky;     // bit lx set <=> prejudge passes in x / y for that lx (binPhy.py:240-241)
     int32_t any_zero;      // maskB has a zero cell -> the window max includes a 0 term
-    int32_t tile;          // 4 / 2: the bottom table is constant on tile x tile blocks (see TileEntry); 1: cell list
+    int32_t tile;          // 4 / 2: the bottom table is constant on tile x tile blocks (see TileEntry); 1: cell list (every
+                           // table of a stepSize-1 handle: the block form needs windows aligned to the blocks)
     double ez;             // round(extent_z, 6)   (space.py:104,120)
     int64_t off;           // offset of Bs / Ts of this entry in the pools (doubles)
     int32_t tile_off;      // first TileEntry of this (shape, rotation)
@@ -96,7 +114,8 @@ struct ShapeRot {          // one (shape, rotation) entry, device resident
 // into the column-parity heightmap planes).  Masked cells / blocks have no entry.
 struct alignas(16) TileEntry {     // 16 bytes: one LDS.128 per entry
     int32_t off;           // BYTE offset added to the pose's base address: 8 * (block du*16 + dv), 8 * cell hm_index(i, j)
-    int32_t pad;
+    int32_t off_odd;       // stepSize 1, cell lists: the offset from a window origin in an odd heightmap row (the column-parity
+                           // planes swap there), 8 * (hm_index(i, j + 1) - hm_index(0, 1)); unused otherwise
     double b;              // bottom height of the block / cell
 };
 
@@ -170,22 +189,22 @@ struct Params {
     int32_t traj_end;                    //   first + count: trajectories from here on are not played
     // per-env state
     double* hm;                          // [N][2][32][16] column-parity planes
-    uint16_t* cand;                      // [N][cand_stride] rot<<8 | x<<4 | y  (rows padded to 16 bytes: bulk-copied)
+    uint16_t* cand;                      // [N][cand_stride] Grid::pack(rot, x, y)  (rows padded to 16 bytes: bulk-copied)
     int32_t cand_stride;                 // uint16 entries per row, sel rounded up to a multiple of 8
     EnvState* state;                     // [N]
     // scan -> candidates hand-over (global scratch, L2 resident)
-    double* posz;                        // [N][R][256] drop heights (posZmap)
-    uint32_t* maskbits;                  // [N][R][8]   feasibility bits (naiveMask)
-    uint32_t* bitmaps;                   // [N][R][MAX_LEVELS][8] level images
+    double* posz;                        // [N][R][NPOSE] drop heights (posZmap)
+    uint32_t* maskbits;                  // [N][R][BMW]   feasibility bits (naiveMask)
+    uint32_t* bitmaps;                   // [N][R][MAX_LEVELS][BMW] level images
     int32_t* nlevels;                    // [N][R]
     // inputs of this call
     const int64_t* actions;              // MODE_STEP / MODE_CANDIDATES
     const uint8_t* which;                // MODE_RESET (NULL = all)
     const int32_t* dbg_items;            // MODE_DEBUG_SCAN
-    uint16_t* dlist;                     // [units][2][R*256] phase D lists of bins with more than LIST_CAP_WS candidates (NULL if R*256 <= LIST_CAP_WS)
+    uint16_t* dlist;                     // [units][2][R*NPOSE] phase D lists of bins with more than LIST_CAP_WS candidates (NULL if R*NPOSE <= LIST_CAP_WS)
     uint32_t* ready;                     // [units] hand-over flags: the scan CTA of a unit stores `epoch` when its scratch is written (NULL: grid-wide wait)
     uint32_t epoch;                      // value of this launch (never 0)
-    int32_t pose_actions;                // MODE_STEP: actions are flat poses (rot*256 + lx*16 + ly), not candidate rows
+    int32_t pose_actions;                // MODE_STEP: actions are flat poses ((rot*AX + lx)*AY + ly), not candidate rows
     int32_t heur_method, heur_dir;       // heuristic kernel: Heuristic, dirIdx 0..3 (space.py:162-166)
     int32_t* heur_pose;                  // [N][3] rot, lx, ly
     int64_t* heur_index;                 // [N] row of that pose in the candidate table, -1 if absent
@@ -197,6 +216,8 @@ struct Params {
     StepResults res_host;                // host-mapped block of a step with host actions (zero-copy stores), else all NULL
     unsigned long long* phase_cycles;    // [8] summed SM cycles per phase (thread 0 of every CTA), or NULL
     int32_t mode;
+    uint8_t* ovf;                        // stepSize 1: [candidates CTAs * EPC] overflow buffers of the contour redo, one per warp
+                                         // (CandScratch::OVF_BYTES each)
 };
 
 // one bin's row of step results, stored to the device block and, when it is set, to the host-mapped block
@@ -301,9 +322,9 @@ __host__ __device__ __forceinline__ bool mode_writes_state(int mode, int slot, i
 }
 
 // ---- scan -> candidates scratch: the slice of unit u (a bin, or a (bin, buffer slot) pair) and rotation r ----------
-__device__ __forceinline__ double* posz_of(const Params& P, int u, int r) { return P.posz + ((int64_t)u * P.R + r) * NPOSE; }
-__device__ __forceinline__ uint32_t* maskbits_of(const Params& P, int u, int r) { return P.maskbits + ((int64_t)u * P.R + r) * 8; }
-__device__ __forceinline__ uint32_t* bitmaps_of(const Params& P, int u, int r) { return P.bitmaps + ((int64_t)u * P.R + r) * MAX_LEVELS * 8; }
+template <class G> __device__ __forceinline__ double* posz_of(const Params& P, int u, int r) { return P.posz + ((int64_t)u * P.R + r) * G::NPOSE; }
+template <class G> __device__ __forceinline__ uint32_t* maskbits_of(const Params& P, int u, int r) { return P.maskbits + ((int64_t)u * P.R + r) * G::BMW; }
+template <class G> __device__ __forceinline__ uint32_t* bitmaps_of(const Params& P, int u, int r) { return P.bitmaps + ((int64_t)u * P.R + r) * MAX_LEVELS * G::BMW; }
 __device__ __forceinline__ int32_t* nlevels_of(const Params& P, int u, int r) { return P.nlevels + (int64_t)u * P.R + r; }
 
 // ---- warp and phase helpers of both step kernels ----------------------------------------------------------------
@@ -347,15 +368,17 @@ __device__ __forceinline__ void mark_level(int L, uint32_t& pres_lo, uint32_t& p
     }
 }
 
-// lv[pass] = level of pose pass*32+lane (or -1), pres_lo / pres_hi = this lane's presence bits.  One 16x16 bitmap (8
-// words, two rows each) per level present in the warp, by warp ballots, written to the scratch with their count.
-__device__ __forceinline__ void emit_level_bitmaps(const Params& P, int u, int r, int lane, const int (&lv)[8],
+// lv(pass) = level of pose pass*32+lane (or -1), pres_lo / pres_hi = this lane's presence bits.  One Ax x Ay bitmap (BMW
+// words: two 16-pixel rows or one 32-pixel row each) per level present in the warp, by warp ballots, written to the
+// scratch with their count.
+template <class G, class LV>
+__device__ __forceinline__ void emit_level_bitmaps(const Params& P, int u, int r, int lane, const LV& lv,
                                                    uint32_t pres_lo, uint32_t pres_hi) {
     pres_lo = __reduce_or_sync(0xffffffffu, pres_lo);
     pres_hi = __reduce_or_sync(0xffffffffu, pres_hi);
     uint64_t present = ((uint64_t)pres_hi << 32) | pres_lo;
     present &= ~(1ull << (LEVEL_OFFSET - 1));        // level -1 is skipped (cvTools.py:84)
-    uint32_t* bm_g = bitmaps_of(P, u, r);
+    uint32_t* bm_g = bitmaps_of<G>(P, u, r);
     int k = 0;
     while (present) {
         const int b = __ffsll((long long)present) - 1;
@@ -363,11 +386,11 @@ __device__ __forceinline__ void emit_level_bitmaps(const Params& P, int u, int r
         const int L = b - LEVEL_OFFSET;
         uint32_t mine = 0;
 #pragma unroll
-        for (int pass = 0; pass < 8; ++pass) {
-            const uint32_t bits = __ballot_sync(0xffffffffu, lv[pass] == L);
+        for (int pass = 0; pass < G::BMW; ++pass) {
+            const uint32_t bits = __ballot_sync(0xffffffffu, lv(pass) == L);
             if (lane == pass) mine = bits;
         }
-        if (lane < 8) bm_g[k * 8 + lane] = mine;
+        if (lane < G::BMW) bm_g[k * G::BMW + lane] = mine;
         ++k;
     }
     if (lane == 0) *nlevels_of(P, u, r) = k;
@@ -382,6 +405,7 @@ __device__ __forceinline__ int level_of(const Params& P, double posz, double inv
 }
 
 // ---- phase B: one warp scans one rotation -------------------------------------------------------------
+// Block form, stepSize 2 only (the blocks are aligned to the 2x2 / 4x4 action windows).
 // Writes posz[r][256], maskbits[r][8], the level bitmaps and their count (space.py:98-129,
 // cvTools.py:78-85).  Returns true if any pose is feasible.
 // `arr` is the array the entry offsets refer to: the block maxima M (pose base = X*16 + Y) for block
@@ -390,6 +414,7 @@ __device__ __forceinline__ int level_of(const Params& P, double posz, double inv
 // (X, Y) and (X + 8, Y), so one entry serves two window positions.
 __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr, int stride_x, TileEntry* es,
                                               int env, int item, int r, int lane, int& err) {
+    using G = Grid<2>;
     const ShapeRot* sr = P.srot + (int64_t)item * P.R + r;
     const int nX = sr->nX, nY = sr->nY, nt = sr->ntiles;
     const double ez = sr->ez;
@@ -401,8 +426,8 @@ __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr
         __syncwarp();
     }
     const double inv = 1.0 / P.resZ;
-    double* posz_g = posz_of(P, env, r);
-    uint32_t* mask_g = maskbits_of(P, env, r);
+    double* posz_g = posz_of<G>(P, env, r);
+    uint32_t* mask_g = maskbits_of<G>(P, env, r);
     int lv[8];
     uint32_t pres_lo = 0, pres_hi = 0, any = 0;
     const int Y = lane & 15;
@@ -438,7 +463,7 @@ __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr
         lv[pass] = feasA ? level_of(P, accA, inv, pres_lo, pres_hi, err) : -1;
         lv[pass + 4] = feasB ? level_of(P, accB, inv, pres_lo, pres_hi, err) : -1;
     }
-    emit_level_bitmaps(P, env, r, lane, lv, pres_lo, pres_hi);
+    emit_level_bitmaps<G>(P, env, r, lane, [&](int pass) { return lv[pass]; }, pres_lo, pres_hi);
     return any != 0;
 }
 
@@ -449,10 +474,13 @@ __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr
 // is where the scan of general shapes spends its time.  Here only the nX * nY scanned poses are dealt to the
 // lanes (pose v -> X = v / nY, Y = v mod nY), four per lane, so one staged entry serves 128 window positions
 // and four independent accumulators hide the latency of the max chain.  Results go to posz as before and, as
-// one level code per pose, to a 256-byte map in shared memory from which a second, fixed-layout pass takes the
+// one level code per pose, to a NPOSE-byte map in shared memory from which a second, fixed-layout pass takes the
 // feasibility bits and the level bitmaps by warp ballots (emit_level_bitmaps).
+// stepSize 2: `arr` + X * stride_x + Y is the pose's base (even window origins: one offset per entry).  stepSize 1: the
+// base is hm_index(X, Y) of the heightmap planes and a pose in an odd row Y takes the entries' off_odd.
+template <class G>
 __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const double* arr, int stride_x, TileEntry* es,
-                                                    uint8_t* lv_s /* [256], this warp's */, int env, int item, int r,
+                                                    uint8_t* lv_s /* [NPOSE], this warp's */, int env, int item, int r,
                                                     int lane, int& err) {
     const ShapeRot* sr = P.srot + (int64_t)item * P.R + r;
     const int nX = sr->nX, nY = sr->nY, nt = sr->ntiles;
@@ -465,18 +493,21 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
         for (int k = lane; k < nt; k += 32) es[k] = te[k];
         reinterpret_cast<uint32_t*>(lv_s)[lane] = 0u;
         reinterpret_cast<uint32_t*>(lv_s)[lane + 32] = 0u;
+#pragma unroll
+        for (int q = 2; q < G::NPOSE / 128; ++q) reinterpret_cast<uint32_t*>(lv_s)[lane + 32 * q] = 0u;
         __syncwarp();
     }
     const double inv = 1.0 / P.resZ;
-    double* posz_g = posz_of(P, env, r);
-    const uint32_t magic = 65536u / (uint32_t)(nY > 0 ? nY : 1) + 1u;      // v / nY == (v * magic) >> 16 for v < 256, nY <= 16
+    double* posz_g = posz_of<G>(P, env, r);
+    // v / nY == (v * magic) >> 16 whenever v * nY < 2^16: v < NPOSE, nY <= AY (256 * 16 and 1024 * 32 are both below 2^16)
+    const uint32_t magic = 65536u / (uint32_t)(nY > 0 ? nY : 1) + 1u;
     // PPL poses per lane: chunks of 128 poses with four accumulators per lane, then what is left (nX * nY is
     // rarely a multiple of 128) with two or one, so the tail does not cost a full four-pose pass
     auto chunk = [&](int c0, auto ppl_tag) {
         constexpr int PPL = decltype(ppl_tag)::value;
         int cell[PPL];
         const char* base[PPL];
-        bool valid[PPL];
+        bool valid[PPL], odd[PPL];
         double acc[PPL];
 #pragma unroll
         for (int k = 0; k < PPL; ++k) {
@@ -484,8 +515,14 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
             valid[k] = v < V;
             const int X = valid[k] ? (int)(((uint32_t)v * magic) >> 16) : 0;
             const int Y = valid[k] ? v - X * nY : 0;
-            cell[k] = X * 16 + Y;
-            base[k] = reinterpret_cast<const char*>(arr + X * stride_x + Y);
+            cell[k] = X * G::AY + Y;
+            if constexpr (G::STEP == 1) {
+                base[k] = reinterpret_cast<const char*>(arr + hm_index(X, Y));
+                odd[k] = (Y & 1) != 0;
+            } else {
+                base[k] = reinterpret_cast<const char*>(arr + X * stride_x + Y);
+                odd[k] = false;
+            }
             acc[k] = init;
         }
 #pragma unroll 2
@@ -493,7 +530,8 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
             const TileEntry en = es[e];
 #pragma unroll
             for (int k = 0; k < PPL; ++k) {
-                const double u = *reinterpret_cast<const double*>(base[k] + en.off) - en.b;      // entry offsets are in bytes
+                const int off = (G::STEP == 1 && odd[k]) ? en.off_odd : en.off;
+                const double u = *reinterpret_cast<const double*>(base[k] + off) - en.b;      // entry offsets are in bytes
                 acc[k] = (u > acc[k]) ? u : acc[k];
             }
         }
@@ -519,23 +557,31 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
         else if (V - c0 > 0) chunk(c0, std::integral_constant<int, 1>());
     }
     __syncwarp();
-    // fixed-layout pass: feasibility bits, level presence, bitmaps; poses outside the scanned range keep 1e3 / 0
-    uint32_t* mask_g = maskbits_of(P, env, r);
-    int lv[8];
+    // fixed-layout pass: feasibility bits, level presence, bitmaps; poses outside the scanned range keep 1e3 / 0.
+    // 16x16: the levels of a lane's 8 poses stay in registers for the ballots; 32x32: 32 poses per lane, the ballots
+    // read them back from the level map
+    uint32_t* mask_g = maskbits_of<G>(P, env, r);
+    constexpr bool LV_REGS = G::BMW <= 8;
+    int lv[LV_REGS ? G::BMW : 1];
     uint32_t pres_lo = 0, pres_hi = 0, any = 0;
 #pragma unroll
-    for (int pass = 0; pass < 8; ++pass) {
+    for (int pass = 0; pass < G::BMW; ++pass) {
         const int pA = pass * 32 + lane;
         const int code = lv_s[pA];
-        if ((pA >> 4) >= nX || (pA & 15) >= nY) posz_g[pA] = POSZ_INVALID;
+        if ((pA >> G::LOG) >= nX || (pA & G::MASK) >= nY) posz_g[pA] = POSZ_INVALID;
         const uint32_t mb = __ballot_sync(0xffffffffu, code != 0);
         if (lane == 0) mask_g[pass] = mb;
         any |= mb;
         const int L = code - (LEVEL_OFFSET + 1);
-        lv[pass] = code ? L : -1;
+        if constexpr (LV_REGS) lv[pass] = code ? L : -1;
         if (code) mark_level(L, pres_lo, pres_hi);
     }
-    emit_level_bitmaps(P, env, r, lane, lv, pres_lo, pres_hi);
+    if constexpr (LV_REGS) {
+        emit_level_bitmaps<G>(P, env, r, lane, [&](int pass) { return lv[pass]; }, pres_lo, pres_hi);
+    } else {
+        emit_level_bitmaps<G>(P, env, r, lane, [&](int pass) { const int code = lv_s[pass * 32 + lane]; return code ? code - (LEVEL_OFFSET + 1) : -1; },
+                              pres_lo, pres_hi);
+    }
     return any != 0;
 }
 
@@ -565,20 +611,22 @@ __device__ __forceinline__ void backoff() { __nanosleep(100); }
 constexpr int READY_POLLS = 1 << 16;       // ~10 ms of polling before the fallback
 
 // ---- scan kernel ------------------------------------------------------------------------------------------
-// TRAJ: the item source is trajectory replay (idle bins exist); the other sources run the instantiation without that code
-template <bool TRAJ>
-__global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(const Params P) {
+// G: the action grid.  TRAJ: the item source is trajectory replay (idle bins exist); the other sources run the
+// instantiation without that code
+template <class G, bool TRAJ>
+__global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : SCAN_MIN_CTAS_FINE)) irbpp_scan_kernel(const Params P) {
     __shared__ __align__(128) double hm_s[HX * HY];
     extern __shared__ __align__(16) TileEntry estage[];  // CTA_WARPS x P.maxwh: scan list of each warp's rotation
     __shared__ __align__(16) EnvState st_s;              // this bin's scalar state (loaded / stored by warp 0)
-    __shared__ double M_s[NPOSE];                        // block maxima of the heightmap (block form of phase B)
-    __shared__ double P2_s[NPOSE];                       // 2x2 block maxima
+    constexpr int NBLK = G::STEP == 2 ? G::NPOSE : 1;    // the block form exists at stepSize 2 only
+    __shared__ double M_s[NBLK];                         // block maxima of the heightmap (block form of phase B)
+    __shared__ double P2_s[NBLK];                        // 2x2 block maxima
     __shared__ double z_sh;
     __shared__ int ok_sh, rot_sh, lx_sh, ly_sh, item_sh, err_sh, any_sh;   // item_sh < 0: the bin is idle (no trajectory left)
     __shared__ __align__(8) mbarrier_t mbar;             // completion of the bulk copies of this bin's inputs
     __shared__ __align__(16) ShapeRot srot_s[MAX_ROT];   // (56 bytes each) table headers of the item the action places (all rotations), prefetched
     __shared__ long long a_sh;                           // the bin's action
-    __shared__ __align__(16) uint8_t lvmap_s[CTA_WARPS * NPOSE];   // per warp: level code of every pose of its rotation (dense scan)
+    __shared__ __align__(16) uint8_t lvmap_s[CTA_WARPS * G::NPOSE];   // per warp: level code of every pose of its rotation (dense scan)
     const int mode = P.mode;
     // One CTA per bin; get_all_possible_observation (MODE_ALL_OBS) runs one CTA per (bin, buffer slot) in a single
     // launch: `vb` indexes the hand-over scratch, the slot picks the item and the place in the observation.
@@ -687,10 +735,10 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
         bool ok = true;
         {
             const int64_t a = a_sh;
-            if (a < 0 || a >= (P.pose_actions ? P.R * NPOSE : P.sel)) { ok = false; if (tid == 0) err_sh = 2; }
+            if (a < 0 || a >= (P.pose_actions ? P.R * G::NPOSE : P.sel)) { ok = false; if (tid == 0) err_sh = 2; }
             else {
                 const uint32_t c = P.pose_actions ? (uint32_t)a : (uint32_t)cand_s[a];
-                rot = c >> 8; lx = (c >> 4) & 15; ly = c & 15;
+                rot = c >> (2 * G::LOG); lx = (c >> G::LOG) & G::MASK; ly = c & G::MASK;
                 if (rot >= P.R) { rot = 0; ok = false; if (tid == 0) err_sh = 2; }
             }
         }
@@ -710,7 +758,7 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
                 double acc = sr.any_zero ? 0.0 : -INFINITY;
                 for (int c = lane; c < w * h; c += 32) {
                     const int i = c / h, j = c - i * h;
-                    const double v = hm_s[hm_index(STEP * lx + i, STEP * ly + j)] - B[c];
+                    const double v = hm_s[hm_index(G::STEP * lx + i, G::STEP * ly + j)] - B[c];
                     acc = (v > acc) ? v : acc;
                 }
 #pragma unroll
@@ -729,7 +777,7 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
         if (ok) {
             // heightmap update: hm[win] = max(hm[win], (T + z) * maskT)   (space.py:213)
             const double z = z_sh;
-            const int x0 = STEP * lx, y0 = STEP * ly;
+            const int x0 = G::STEP * lx, y0 = G::STEP * ly;
             // only the cells the item raises are written back (in shared and in global memory): a placement
             // touches at most w x h cells, the other 8 KB of the bin's heightmap stay as they are in HBM
             for (int c = tid; c < w * h; c += CTA_THREADS) {
@@ -805,10 +853,10 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
         int err = 0;
         bool any = false;
         const int tile = P.srot[(int64_t)item * P.R].tile;      // same for every rotation of a shape
-        if (tile > 1) {
+        if (G::STEP == 2 && tile > 1) {
             // block maxima of the heightmap, one entry per action-grid offset.  max is exact, so the
             // 4x4 maximum is taken as the maximum of four 2x2 maxima (8 loads per entry instead of 16).
-            for (int e = tid; e < NPOSE; e += CTA_THREADS) {
+            for (int e = tid; e < NBLK; e += CTA_THREADS) {
                 const double* p0 = hm_s + (2 * (e >> 4)) * (HY / 2) + (e & 15);     // plane of even y, row x = 2a
                 const double* p1 = p0 + HX * (HY / 2);                              // plane of odd y
                 const double m0 = (p0[0] > p0[HY / 2]) ? p0[0] : p0[HY / 2];
@@ -817,9 +865,9 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
             }
             __syncthreads();
             if (tile == 4) {
-                for (int e = tid; e < NPOSE; e += CTA_THREADS) {
+                for (int e = tid; e < NBLK; e += CTA_THREADS) {
                     double m = -INFINITY;
-                    if ((e >> 4) < AX - 1 && (e & 15) < AY - 1) {
+                    if ((e >> 4) < Grid<2>::AX - 1 && (e & 15) < Grid<2>::AY - 1) {
                         const double m0 = (P2_s[e] > P2_s[e + 1]) ? P2_s[e] : P2_s[e + 1];
                         const double m1 = (P2_s[e + 16] > P2_s[e + 17]) ? P2_s[e + 16] : P2_s[e + 17];
                         m = (m0 > m1) ? m0 : m1;
@@ -833,7 +881,8 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
                 any |= scan_rotation(P, Marr, 16, estage + warp * P.maxwh, vb, item, r, lane, err);
         } else {
             for (int r = warp; r < P.R; r += CTA_WARPS)
-                any |= scan_rotation_dense(P, hm_s, STEP * (HY / 2), estage + warp * P.maxwh, lvmap_s + warp * NPOSE, vb, item, r, lane, err);
+                any |= scan_rotation_dense<G>(P, hm_s, G::STEP * (HY / 2), estage + warp * P.maxwh, lvmap_s + warp * G::NPOSE, vb, item, r,
+                                              lane, err);
         }
         if (lane == 0 && any) any_sh = 1;
         if (__any_sync(0xffffffffu, err) && lane == 0) err_sh = 4;
@@ -878,6 +927,7 @@ __global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_kernel(
 
 
 // ---- levels kernel (MODE_DEBUG_HULLS): level bitmaps from caller-supplied posZValid / mask ------------------
+template <class G>
 __global__ void __launch_bounds__(CTA_THREADS) irbpp_levels_kernel(const Params P) {
     __shared__ int err_sh;
     const int env = P.env_lo + blockIdx.x;
@@ -887,16 +937,16 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_levels_kernel(const Params 
     __syncthreads();
     int err = 0;
     for (int r = warp; r < P.R; r += CTA_WARPS) {
-        const double* posz_g = posz_of(P, env, r);
-        const uint32_t* mask_g = maskbits_of(P, env, r);
-        int lv[8];
+        const double* posz_g = posz_of<G>(P, env, r);
+        const uint32_t* mask_g = maskbits_of<G>(P, env, r);
+        int lv[G::BMW];
         uint32_t pres_lo = 0, pres_hi = 0;
 #pragma unroll
-        for (int pass = 0; pass < 8; ++pass) {
+        for (int pass = 0; pass < G::BMW; ++pass) {
             const bool feas = (mask_g[pass] >> lane) & 1u;
             lv[pass] = feas ? level_of(P, posz_g[pass * 32 + lane], inv, pres_lo, pres_hi, err) : -1;
         }
-        emit_level_bitmaps(P, env, r, lane, lv, pres_lo, pres_hi);
+        emit_level_bitmaps<G>(P, env, r, lane, [&](int pass) { return lv[pass]; }, pres_lo, pres_hi);
     }
     if (err) err_sh = 4;
     __syncthreads();
@@ -907,6 +957,7 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_levels_kernel(const Params 
 // One CTA per bin over the scan scratch of the bin's current item: every thread scores the poses
 // e = tid, tid + 128, ... (flat (rot, lx, ly) order), then a lexicographic (score, e) minimum gives
 // np.argmin's first-minimum pose.  Also looks the pose up in the bin's candidate table.
+template <class G>
 __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Params P) {
     __shared__ __align__(16) double hm_s[HX * HY];
     __shared__ double best_sh[CTA_WARPS];
@@ -933,14 +984,14 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
     auto hm_at = [&](int x, int y) { return hm_s[hm_index(x, y)]; };
     double best = INFINITY;
     int beste = 0x7fffffff;
-    for (int e = tid; e < P.R * NPOSE; e += CTA_THREADS) {
-        const int r = e >> 8, p = e & 255;
-        const bool feas = (maskbits_of(P, env, r)[p >> 5] >> (p & 31)) & 1u;
+    for (int e = tid; e < P.R * G::NPOSE; e += CTA_THREADS) {
+        const int r = e >> (2 * G::LOG), p = e & (G::NPOSE - 1);
+        const bool feas = (maskbits_of<G>(P, env, r)[p >> 5] >> (p & 31)) & 1u;
         double s = HEUR_INVALID;
         if (feas) {
             const ShapeRot* sr = P.srot + (int64_t)item * P.R + r;
-            const double z = posz_of(P, env, r)[p];
-            s = heuristic_score(method, P.heur_dir, p >> 4, p & 15, z, P.resA, AX, AY, STEP, hm_at,
+            const double z = posz_of<G>(P, env, r)[p];
+            s = heuristic_score(method, P.heur_dir, p >> G::LOG, p & G::MASK, z, P.resA, G::AX, G::AY, G::STEP, hm_at,
                                 P.Ts + sr->off, sr->w, sr->h);
         }
         if (s < best) { best = s; beste = e; }
@@ -966,9 +1017,9 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
     if (first != 0x7fffffff) atomicMin(&idx_sh, first);
     __syncthreads();
     if (tid == 0) {
-        P.heur_pose[env * 3 + 0] = beste >> 8;
-        P.heur_pose[env * 3 + 1] = (beste >> 4) & 15;
-        P.heur_pose[env * 3 + 2] = beste & 15;
+        P.heur_pose[env * 3 + 0] = beste >> (2 * G::LOG);
+        P.heur_pose[env * 3 + 1] = (beste >> G::LOG) & G::MASK;
+        P.heur_pose[env * 3 + 2] = beste & G::MASK;
         P.heur_index[env] = (idx_sh == 0x7fffffff) ? -1 : idx_sh;
     }
 }
@@ -979,27 +1030,42 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
 // that the lanes of a warp carry images of similar size -- the lanes run in lock step and a warp costs
 // what its heaviest lane costs (the floor-level image of each rotation is an order of magnitude
 // heavier than the small plateaus above it).
-// Per-warp scratch of the candidates kernel, 3 KB for every rotation count: in phase C the lane-strided contour points of
-// the task slots (FAST_CAP points for slot 0, SLOT_CAP for the others) and the 1024-point overflow buffers; in phase D the
+// Per-warp scratch of the candidates kernel, 3 KB per contour-point byte for every rotation count (3 KB on the 16x16 grid,
+// 6 KB on the 32x32 grid, whose points take two bytes): in phase C the lane-strided contour points of the task slots
+// (FAST_CAP points for slot 0, SLOT_CAP for the others) and, on the 16x16 grid, the overflow buffer; in phase D the
 // candidate list + its bucket-sorted entry list (2 x uint16 per candidate).  A bin with more than LIST_CAP_WS candidates
 // (BlockOut bins of the bench workload have at most ~210 of the 1024 possible at R = 4) spills its lists to a global
 // scratch (Params::dlist, L2 resident).  A scratch sized for the worst case would decide the residency instead (4 KB per
 // warp at R = 4 left seven 4-bin CTAs per SM: 924 on 132 SMs, so 4096 bins took a second wave).
-constexpr int WS_BYTES = 3072;
-constexpr int LIST_CAP_WS = WS_BYTES / 4;                // candidates whose lists fit the warp scratch
-constexpr int SLOT_CAP_FIT = TASKS_PER_LANE > 1 ? (WS_BYTES - FAST_CAP * 32) / ((TASKS_PER_LANE - 1) * 32) : FAST_CAP;
-constexpr int SLOT_CAP = SLOT_CAP_FIT < FAST_CAP ? SLOT_CAP_FIT : FAST_CAP;     // contour points of task slots 1.. (slot 0: FAST_CAP)
-static_assert(WS_BYTES % 16 == 0 && WS_BYTES >= 2 * BIG_CAP, "the serial overflow redo lays two 1024-point buffers over the warp scratch");
-static_assert(SLOT_CAP >= 16 && FAST_CAP * 32 + (TASKS_PER_LANE - 1) * SLOT_CAP * 32 <= WS_BYTES,
-              "the task slots' point buffers share the warp scratch");
+// The overflow redo follows a contour with BIG_CAP points: a border passes every pixel at most four times (once per side),
+// so 4 * NPOSE points hold any contour and IRBPP_EDEVICE code 6 cannot occur.  At 32x32 that buffer (4096 two-byte points
+// and their kept flags, 12 KB) does not fit the warp scratch and lives in a global scratch, one per warp of every CTA (Params::ovf): the idle warps of a
+// partial last CTA take contour tasks in phase C too.
+template <class G>
+struct CandScratch {
+    static constexpr int PT_BYTES = (int)sizeof(typename G::Img::Point);
+    static constexpr int WS_BYTES = 3072 * PT_BYTES;
+    static constexpr int LIST_CAP_WS = WS_BYTES / 4;                 // candidates whose lists fit the warp scratch
+    static constexpr int SLOT_CAP_FIT = TASKS_PER_LANE > 1 ? (WS_BYTES - FAST_CAP * 32 * PT_BYTES) / ((TASKS_PER_LANE - 1) * 32 * PT_BYTES) : FAST_CAP;
+    static constexpr int SLOT_CAP = SLOT_CAP_FIT < FAST_CAP ? SLOT_CAP_FIT : FAST_CAP;     // contour points of task slots 1.. (slot 0: FAST_CAP)
+    static constexpr int BIG_CAP = 4 * G::NPOSE;
+    using Big = FlatScratch<BIG_CAP, G::LOG>;
+    static constexpr bool OVF_GLOBAL = Big::BYTES > WS_BYTES;
+    static constexpr int OVF_BYTES = (Big::BYTES + 15) & ~15;
+    static_assert(WS_BYTES % 16 == 0, "warp scratches are 16-byte aligned");
+    static_assert(SLOT_CAP >= 16 && (FAST_CAP + (TASKS_PER_LANE - 1) * SLOT_CAP) * 32 * PT_BYTES <= WS_BYTES,
+                  "the task slots' point buffers share the warp scratch");
+};
+static_assert(!CandScratch<Grid<2>>::OVF_GLOBAL, "16x16 grid: the serial overflow redo lays its 1024-point buffer over the warp scratch");
 constexpr int RANK_BUCKETS = 256;                        // height buckets of the phase-D truncation ranking (per warp: bases + cursors)
 static_assert(RANK_BUCKETS % 32 == 0 && 32 * ROWS_WORDS >= 2 * RANK_BUCKETS, "phase D's rank histograms reuse the image slots (one warp's share each)");
 
-template <int EPC>
+template <int EPC, class G>
 struct CandSmem {
     static constexpr int ENVS_PER_CTA = EPC, CAND_WARPS = EPC, CAND_THREADS = 32 * EPC;
-    uint32_t slots[CAND_THREADS * ROWS_WORDS];            // level images of this round in padded row form (one per thread)
-    uint16_t task_tab[TASK_TAB];                          // micro-task m < TASK_TAB: slot << 8 | x << 4 | y of its start pixel
+    using TaskEntry = typename std::conditional<G::LOG == 4, uint16_t, uint32_t>::type;
+    uint32_t slots[CAND_THREADS * G::Img::ROWS_WORDS];    // level images of this round in padded row form (one per thread)
+    TaskEntry task_tab[TASK_TAB];                         // micro-task m < TASK_TAB: slot << 2 LOG | x << LOG | y of its start pixel
     int32_t pre[ENVS_PER_CTA * MAX_ROT + 1];              // prefix of level counts over (bin, rotation)
     int32_t cand_off[CAND_THREADS + 1];                   // prefix of start-candidate counts over the images, in cost order
     uint16_t slot_of[CAND_THREADS];                       // image slot at each position of the cost order
@@ -1012,27 +1078,38 @@ struct CandSmem {
     int32_t error[ENVS_PER_CTA];
 };
 
-// Dynamic shared memory of a candidates CTA: the fixed part, EPC warp scratches, the 256-bit candidate sets per (bin, rotation).
-template <int EPC>
+// Dynamic shared memory of a candidates CTA: the fixed part, EPC warp scratches, the NPOSE-bit candidate sets per (bin, rotation).
+template <int EPC, class G>
 __host__ __device__ constexpr int cand_smem_bytes(int R) {
-    return (int)((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15) + EPC * WS_BYTES + EPC * R * 8 * 4;
+    return (int)((sizeof(CandSmem<EPC, G>) + 15) & ~(size_t)15) + EPC * CandScratch<G>::WS_BYTES + EPC * R * G::BMW * 4;
 }
-// Residency the candidates kernel is built for: 32 warps per SM, i.e. 8 CTAs of 4 bins or 4 of 8 -- 1056 / 528 CTA slots on
-// 132 SMs, so a 4096-bin grid (1024 / 512 CTAs) runs in one wave.  The register budget (64 per thread) is enforced through
-// __launch_bounds__, the shared-memory budget below: 228 KB per sm_90 SM, of which the hardware reserves 1 KB per CTA.
-template <int EPC>
-__host__ __device__ constexpr int cand_min_ctas() { return 32 / EPC; }
+// Residency the candidates kernel is built for.  16x16 grid: 32 warps per SM, i.e. 8 CTAs of 4 bins or 4 of 8 -- 1056 / 528
+// CTA slots on 132 SMs, so a 4096-bin grid (1024 / 512 CTAs) runs in one wave.  32x32 grid: 16 warps per SM (4 CTAs of 4
+// bins, 2 of 8).  Shared memory decides it there: a thread's image in padded row form is 140 bytes instead of 76 and a
+// warp's scratch 6 KB instead of 3, so a 4-bin CTA needs ~48 KB at R = 2 and 32 warps would need twice the 228 KB of an
+// SM; 16 warps leave each thread up to 128 registers for the longer contours, and 4096 bins take two waves.  The
+// register budget is enforced through __launch_bounds__, the shared-memory budget below: 228 KB per sm_90 SM, of which
+// the hardware reserves 1 KB per CTA.
+template <int EPC, class G>
+__host__ __device__ constexpr int cand_min_ctas() { return (G::STEP == 2 ? 32 : 16) / EPC; }
 constexpr int SM90_SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;
-static_assert(cand_min_ctas<ENVS_PER_CTA_NARROW>() * (cand_smem_bytes<ENVS_PER_CTA_NARROW>(WIDE_MIN_R - 1) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
-              "narrow candidates CTAs at their largest rotation count must fit 32 warps per SM");
-static_assert(cand_min_ctas<ENVS_PER_CTA_WIDE>() * (cand_smem_bytes<ENVS_PER_CTA_WIDE>(WIDE_MIN_R) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
-              "wide candidates CTAs at their smallest rotation count must fit 32 warps per SM");
+template <class G>
+constexpr bool cand_smem_fits() {
+    return cand_min_ctas<ENVS_PER_CTA_NARROW, G>() * (cand_smem_bytes<ENVS_PER_CTA_NARROW, G>(WIDE_MIN_R - 1) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM &&
+           cand_min_ctas<ENVS_PER_CTA_WIDE, G>() * (cand_smem_bytes<ENVS_PER_CTA_WIDE, G>(WIDE_MIN_R) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM;
+}
+static_assert(cand_smem_fits<Grid<2>>(), "16x16 grid: narrow CTAs at their largest and wide CTAs at their smallest rotation count must fit 32 warps per SM");
+static_assert(cand_smem_fits<Grid<1>>(), "32x32 grid: narrow CTAs at their largest and wide CTAs at their smallest rotation count must fit 16 warps per SM");
 
-template <int EPC, bool TRAJ>      // TRAJ: as in irbpp_scan_kernel
-__global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidates_kernel(const Params P) {
+template <int EPC, class G, bool TRAJ>      // G, TRAJ: as in irbpp_scan_kernel
+__global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_candidates_kernel(const Params P) {
     constexpr int ENVS_PER_CTA = EPC, CAND_WARPS = EPC, CAND_THREADS = 32 * EPC;     // one warp per bin
+    using CS = CandScratch<G>;
+    using Img = typename G::Img;
+    using Point = typename Img::Point;
+    constexpr int WS_BYTES = CS::WS_BYTES, ROWS_WORDS = Img::ROWS_WORDS, LOG = G::LOG, MASK = G::MASK;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    CandSmem<EPC>& S = *reinterpret_cast<CandSmem<EPC>*>(smem_raw);
+    CandSmem<EPC, G>& S = *reinterpret_cast<CandSmem<EPC, G>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int env0 = P.env_lo + blockIdx.x * ENVS_PER_CTA;
     const int nenv = min(ENVS_PER_CTA, P.env_hi - env0);
@@ -1077,9 +1154,9 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         for (int i = head + 4 * nvec + lane; i < count; i += 32) z0[i] = 0.0f;
     };
 
-    // dynamic tail: CAND_WARPS blocks of WS_BYTES, then the 256-bit candidate sets per (bin, rotation)
-    uint32_t* candbits = reinterpret_cast<uint32_t*>(smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15) + (size_t)CAND_WARPS * WS_BYTES);
-    for (int i = tid; i < ENVS_PER_CTA * R * 8; i += CAND_THREADS) candbits[i] = 0u;
+    // dynamic tail: CAND_WARPS blocks of WS_BYTES, then the NPOSE-bit candidate sets per (bin, rotation)
+    uint32_t* candbits = reinterpret_cast<uint32_t*>(smem_raw + ((sizeof(CandSmem<EPC, G>) + 15) & ~(size_t)15) + (size_t)CAND_WARPS * WS_BYTES);
+    for (int i = tid; i < ENVS_PER_CTA * R * G::BMW; i += CAND_THREADS) candbits[i] = 0u;
     if (tid < ENVS_PER_CTA) S.error[tid] = 0;
     if (warp == 0) {   // prefix of the level counts over the (bin, rotation) pairs, 32 pairs per step
         int carry = 0;
@@ -1095,7 +1172,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
     }
     __syncthreads();
     const int nimg = S.pre[npairs];
-    unsigned char* ws_base = smem_raw + ((sizeof(CandSmem<EPC>) + 15) & ~(size_t)15);     // CAND_WARPS blocks of WS_BYTES
+    unsigned char* ws_base = smem_raw + ((sizeof(CandSmem<EPC, G>) + 15) & ~(size_t)15);     // CAND_WARPS blocks of WS_BYTES
     uint8_t* W_pts = ws_base + (size_t)warp * WS_BYTES;
 
     // ---- phase C: rounds of CAND_THREADS level images; inside a round one (image, start pixel) per lane ----
@@ -1104,32 +1181,55 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         // 1. thread t loads image t, counts its start candidates (background at W, NW, N, NE) and a cost key
         //    (foreground/background transitions ~ border length)
         int cnt = 0, bucket = 63, my_off = 0;
-        uint32_t sm[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};   // start-pixel masks of this thread's image, two 16-bit rows per word
+        uint32_t sm[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};   // 16x16: start-pixel masks of this thread's image, two 16-bit rows per word
         if (tid < 64) S.hist[tid] = 0;
         __syncthreads();
         if (tid < nround) {
             const int t = base + tid;
             int lo = 0, hi = npairs;                        // pre[lo] <= t < pre[hi]
             while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (S.pre[mid] <= t) lo = mid; else hi = mid; }
-            const uint4* src = reinterpret_cast<const uint4*>(bitmaps_of(P, env0, 0) + ((int64_t)lo * MAX_LEVELS + (t - S.pre[lo])) * 8);
-            const uint4 a = src[0], b = src[1];
-            uint32_t* rows = S.slots + tid * ROWS_WORDS;
-            S.pair_of[tid] = (uint16_t)lo;
-            const uint32_t wv[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-            rows[0] = 0u; rows[17] = 0u;
+            const uint4* src = reinterpret_cast<const uint4*>(bitmaps_of<G>(P, env0, 0) + ((int64_t)lo * MAX_LEVELS + (t - S.pre[lo])) * G::BMW);
+            if constexpr (LOG == 4) {
+                const uint4 a = src[0], b = src[1];
+                uint32_t* rows = S.slots + tid * ROWS_WORDS;
+                S.pair_of[tid] = (uint16_t)lo;
+                const uint32_t wv[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                rows[0] = 0u; rows[17] = 0u;
 #pragma unroll
-            for (int k = 0; k < 8; ++k) { rows[1 + 2 * k] = (wv[k] & 0xFFFFu) << 1; rows[2 + 2 * k] = (wv[k] >> 16) << 1; }
-            uint32_t up = 0;
-            int key = 0;
+                for (int k = 0; k < 8; ++k) { rows[1 + 2 * k] = (wv[k] & 0xFFFFu) << 1; rows[2 + 2 * k] = (wv[k] >> 16) << 1; }
+                uint32_t up = 0;
+                int key = 0;
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                const uint32_t r0 = wv[k] & 0xFFFFu, r1 = wv[k] >> 16;
-                sm[k] = start_mask(r0, up) | (start_mask(r1, r0) << 16);
-                cnt += __popc(sm[k]);
-                key += __popc(r0 ^ (r0 << 1)) + __popc(r1 ^ (r1 << 1)) + __popc(r0 ^ up) + __popc(r1 ^ r0);
-                up = r1;
+                for (int k = 0; k < 8; ++k) {
+                    const uint32_t r0 = wv[k] & 0xFFFFu, r1 = wv[k] >> 16;
+                    sm[k] = start_mask(r0, up) | (start_mask(r1, r0) << 16);
+                    cnt += __popc(sm[k]);
+                    key += __popc(r0 ^ (r0 << 1)) + __popc(r1 ^ (r1 << 1)) + __popc(r0 ^ up) + __popc(r1 ^ r0);
+                    up = r1;
+                }
+                bucket = 63 - min(63, key >> 2);            // bucket 0 = longest borders
+            } else {
+                // one 32-pixel row per word; the start masks are taken again from the rows when the table is filled
+                uint32_t* rows = S.slots + tid * ROWS_WORDS;
+                S.pair_of[tid] = (uint16_t)lo;
+                rows[0] = 0u; rows[33] = 0u;
+                uint32_t up = 0;
+                int key = 0;
+#pragma unroll 2
+                for (int k = 0; k < 8; ++k) {
+                    const uint4 a = src[k];
+                    const uint32_t wv[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const uint32_t r0 = wv[j];
+                        rows[1 + 4 * k + j] = r0;
+                        cnt += __popc(start_mask<32>(r0, up));
+                        key += __popc(r0 ^ (r0 << 1)) + __popc(r0 ^ up);
+                        up = r0;
+                    }
+                }
+                bucket = 63 - min(63, key >> 2);
             }
-            bucket = 63 - min(63, key >> 2);                // bucket 0 = longest borders
             my_off = atomicAdd(&S.hist[bucket], 1);
         }
         __syncthreads();
@@ -1159,13 +1259,25 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         // micro-task lane finds its pixel with one load
         if (tid < nround && cnt > 0) {
             int off = S.cand_off[my_pos];
+            if constexpr (LOG == 4) {
 #pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                uint32_t c = sm[k];
-                while (c && off < TASK_TAB) {
-                    const int b = __ffs((int)c) - 1;           // bit b: column b & 15 of row 2k + (b >> 4)
-                    c &= c - 1;
-                    S.task_tab[off++] = (uint16_t)((tid << 8) | ((b & 15) << 4) | (2 * k + (b >> 4)));
+                for (int k = 0; k < 8; ++k) {
+                    uint32_t c = sm[k];
+                    while (c && off < TASK_TAB) {
+                        const int b = __ffs((int)c) - 1;           // bit b: column b & 15 of row 2k + (b >> 4)
+                        c &= c - 1;
+                        S.task_tab[off++] = (uint16_t)((tid << 8) | ((b & 15) << 4) | (2 * k + (b >> 4)));
+                    }
+                }
+            } else {
+                const uint32_t* rows = S.slots + tid * ROWS_WORDS;
+                for (int y = 0; y < G::AY && off < TASK_TAB; ++y) {
+                    uint32_t c = start_candidates_rows<LOG>(rows, y);
+                    while (c && off < TASK_TAB) {
+                        const int x = __ffs((int)c) - 1;
+                        c &= c - 1;
+                        S.task_tab[off++] = (uint32_t)((tid << (2 * LOG)) | (x << LOG) | y);
+                    }
                 }
             }
         }
@@ -1181,10 +1293,11 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         constexpr int BATCH = CAND_THREADS * TPL;
         auto slot_scratch = [&](int owner) {               // point buffer of task slot `owner` (j * CAND_THREADS + thread)
             const int jj = owner / CAND_THREADS, th = owner - jj * CAND_THREADS;
-            return ws_base + (size_t)(th >> 5) * WS_BYTES + (jj == 0 ? 0 : FAST_CAP * 32 + (jj - 1) * SLOT_CAP * 32) + (th & 31);
+            return reinterpret_cast<Point*>(ws_base + (size_t)(th >> 5) * WS_BYTES +
+                                            (jj == 0 ? 0 : (FAST_CAP * 32 + (jj - 1) * CS::SLOT_CAP * 32) * CS::PT_BYTES)) + (th & 31);
         };
         for (int mb = 0; mb < ntask; mb += BATCH) {
-            int tk[TPL];                                    // slot << 8 | x << 4 | y of my tasks, -1: none
+            int tk[TPL];                                    // slot << 2 LOG | x << LOG | y of my tasks, -1: none
             int npts_j[TPL];
             uint32_t ovf_bits = 0;
 #pragma unroll
@@ -1194,28 +1307,28 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                 int slot = 0, x = 0, y = 0;
                 if (has && m < TASK_TAB) {
                     const int t = S.task_tab[m];
-                    slot = t >> 8; x = (t >> 4) & 15; y = t & 15;
+                    slot = t >> (2 * LOG); x = (t >> LOG) & MASK; y = t & MASK;
                 } else if (has) {                               // beyond the table: search the prefix and the image
                     int lo = 0, hi = CAND_THREADS;              // cand_off[lo] <= m < cand_off[hi]
                     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (S.cand_off[mid] <= m) lo = mid; else hi = mid; }
                     slot = S.slot_of[lo];
                     int k = m - S.cand_off[lo];
                     const uint32_t* ri = S.slots + slot * ROWS_WORDS;
-                    for (y = 0; y < 16; ++y) {
-                        const uint32_t c = start_candidates_rows(ri, y);
+                    for (y = 0; y < G::AY; ++y) {
+                        const uint32_t c = start_candidates_rows<LOG>(ri, y);
                         const int pc = __popc(c);
                         if (k < pc) { x = (int)__fns(c, 0u, k + 1); break; }
                         k -= pc;
                     }
                 }
-                tk[jt] = has ? ((slot << 8) | (x << 4) | y) : -1;
+                tk[jt] = has ? ((slot << (2 * LOG)) | (x << LOG) | y) : -1;
                 // (a) the lane follows the border; the points stay in the task slot's scratch
                 int n = -2, area2 = 1;
                 if (has) {
-                    StridedScratch<32, FAST_CAP> sc;
+                    StridedScratch<32, FAST_CAP, LOG> sc;
                     sc.b = slot_scratch(jt * CAND_THREADS + tid);
                     sc.kept = 0;
-                    n = follow_outer_rows(sc, S.slots + slot * ROWS_WORDS, x, y, area2, jt == 0 ? FAST_CAP : SLOT_CAP);
+                    n = follow_outer_rows(sc, S.slots + slot * ROWS_WORDS, x, y, area2, jt == 0 ? FAST_CAP : CS::SLOT_CAP);
                 }
                 const bool keep = has && n != -2 && area2 <= 0;        // a raster-first start of an outer border
                 if (keep && n < 0) ovf_bits |= 1u << jt;
@@ -1230,7 +1343,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
             for (int jt = 0; jt < TPL; ++jt) {
                 boff[jt] = atomicAdd(&S.hist[63 - min(63, npts_j[jt])], 1);
                 S.n_of[jt * CAND_THREADS + tid] = (uint8_t)npts_j[jt];
-                S.q_of[jt * CAND_THREADS + tid] = (uint16_t)(tk[jt] >= 0 ? S.pair_of[tk[jt] >> 8] : 0);
+                S.q_of[jt * CAND_THREADS + tid] = (uint16_t)(tk[jt] >= 0 ? S.pair_of[tk[jt] >> (2 * LOG)] : 0);
             }
             __syncthreads();
             if (warp == 0) bucket_prefix64(S.hist, S.hbase, lane);
@@ -1245,17 +1358,17 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                 const int owner = S.order2[jt * CAND_THREADS + tid];
                 const int on = S.n_of[owner];
                 if (on > 0) {
-                    StridedScratch<32, FAST_CAP> sc;
+                    StridedScratch<32, FAST_CAP, LOG> sc;
                     sc.b = slot_scratch(owner);
                     sc.kept = 0;
-                    uint32_t* cb = candbits + (int)S.q_of[owner] * 8;
+                    uint32_t* cb = candbits + (int)S.q_of[owner] * G::BMW;
                     approx_and_emit(sc, on, P.legacy != 0,
-                                    [&](int ex, int ey) { const int b = ex * 16 + ey; atomicOr(cb + (b >> 5), 1u << (b & 31)); });
+                                    [&](int ex, int ey) { const int b = ex * G::AY + ey; atomicOr(cb + (b >> 5), 1u << (b & 31)); });
                 }
             }
             __syncthreads();           // scratch of every lane is free again
-            // rare: a contour longer than its slot's buffer; the lanes concerned redo it one at a time with
-            // 1024-point buffers laid over the (now idle) scratch of this warp
+            // rare: a contour longer than its slot's buffer; the lanes concerned redo it one at a time with a
+            // BIG_CAP-point buffer laid over the (now idle) scratch of this warp (16x16) or in the unit's global one (32x32)
 #pragma unroll 1
             for (int jt = 0; jt < TPL; ++jt) {
                 uint32_t ovf = __ballot_sync(0xffffffffu, (ovf_bits >> jt) & 1u);
@@ -1264,12 +1377,13 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                     ovf &= ovf - 1;
                     if (lane == src_lane) {
                         if (P.phase_cycles) atomicAdd(P.phase_cycles + 7, 1ull);     // overflow redo counter
-                        FlatScratch<BIG_CAP> bs;
-                        bs.b = W_pts;
-                        const int slot = tk[jt] >> 8, q = S.pair_of[slot];
-                        uint32_t* cb = candbits + q * 8;
-                        if (!process_start_candidate(bs, S.slots + slot * ROWS_WORDS, (tk[jt] >> 4) & 15, tk[jt] & 15, P.legacy != 0,
-                                [&](int ex, int ey) { const int b = ex * 16 + ey; atomicOr(cb + (b >> 5), 1u << (b & 31)); }))
+                        typename CS::Big bs;
+                        if constexpr (CS::OVF_GLOBAL) bs.b = P.ovf + ((int64_t)blockIdx.x * EPC + warp) * CS::OVF_BYTES;
+                        else bs.b = W_pts;
+                        const int slot = tk[jt] >> (2 * LOG), q = S.pair_of[slot];
+                        uint32_t* cb = candbits + q * G::BMW;
+                        if (!process_start_candidate(bs, S.slots + slot * ROWS_WORDS, (tk[jt] >> LOG) & MASK, tk[jt] & MASK, P.legacy != 0,
+                                [&](int ex, int ey) { const int b = ex * G::AY + ey; atomicOr(cb + (b >> 5), 1u << (b & 31)); }))
                             atomicMax(&S.error[q / R], 6);
                     }
                     __syncwarp();
@@ -1292,9 +1406,9 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
     const int dev_err = S.error[warp];
     // ---- phase D ----
     const int sel = P.sel;
-    const uint32_t* cbits = candbits + warp * R * 8;
-    const uint32_t* mask_g = maskbits_of(P, env, 0);
-    const double* posz_g = posz_of(P, env, 0);
+    const uint32_t* cbits = candbits + warp * R * G::BMW;
+    const uint32_t* mask_g = maskbits_of<G>(P, env, 0);
+    const double* posz_g = posz_of<G>(P, env, 0);
     const int renv = real_env(env);
     float* obs_g = P.obs + obs_offset(env);
     uint16_t* cand_g = mode_writes_state(P.mode, slot_of_e(env), P.K) ? P.cand + (int64_t)renv * P.cand_stride : nullptr;
@@ -1302,18 +1416,18 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
 
     // candidate counts per rotation (lane r), exclusive prefix, total
     int cnt = 0;
-    if (lane < R) { for (int qd = 0; qd < 8; ++qd) cnt += __popc(cbits[lane * 8 + qd]); }
+    if (lane < R) { for (int qd = 0; qd < G::BMW; ++qd) cnt += __popc(cbits[lane * G::BMW + qd]); }
     const int incl = warp_inclusive_scan(cnt, lane);
     const int excl = incl - cnt;
     const int Ktot = __shfl_sync(0xffffffffu, incl, 31);
     uint32_t anym = 0;
-    for (int qd = lane; qd < R * 8; qd += 32) anym |= mask_g[qd];
+    for (int qd = lane; qd < R * G::BMW; qd += 32) anym |= mask_g[qd];
     anym = __reduce_or_sync(0xffffffffu, anym);
 
     auto put_row = [&](int row, int rot, int x, int y, double H, double V) {
         float* d = obs_g + row * 5;
         d[0] = (float)rot; d[1] = (float)x; d[2] = (float)y; d[3] = (float)H; d[4] = (float)V;
-        if (cand_g) cand_g[row] = (uint16_t)((rot << 8) | (x << 4) | y);
+        if (cand_g) cand_g[row] = (uint16_t)G::pack(rot, x, y);
         if (dbg_cand) { double* qd = dbg_cand + row * 5; qd[0] = rot; qd[1] = x; qd[2] = y; qd[3] = H; qd[4] = V; }
     };
     auto zero_rows = [&](int first) {
@@ -1328,10 +1442,10 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
 
     if (Ktot == 0) {
         // no hull candidate at all (binPhy.py:217-225): the `sel` smallest posZValid, stable order
-        const int total = R * NPOSE;
+        const int total = R * G::NPOSE;
         if (!anym) {
             const int nrow = total < sel ? total : sel;
-            for (int i = lane; i < nrow; i += 32) put_row(i, i >> 8, (i >> 4) & 15, i & 15, P.binz, 0.0);
+            for (int i = lane; i < nrow; i += 32) put_row(i, i >> (2 * LOG), (i >> LOG) & MASK, i & MASK, P.binz, 0.0);
             zero_rows(nrow);
         } else {
             for (int i = lane; i < total; i += 32) {
@@ -1341,7 +1455,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                     bool mj; const double vj = height_of(j, mj);
                     rank += (vj < vi) || (vj == vi && j < i);
                 }
-                if (rank < sel) put_row(rank, i >> 8, (i >> 4) & 15, i & 15, P.binz, mi ? 1.0 : 0.0);
+                if (rank < sel) put_row(rank, i >> (2 * LOG), (i >> LOG) & MASK, i & MASK, P.binz, mi ? 1.0 : 0.0);
             }
             zero_rows(total < sel ? total : sel);
         }
@@ -1351,20 +1465,21 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
         // candidate, so the height gathers of 32 candidates are in flight together.
         // candidate list + bucket-sorted index list: the (now idle) lane scratch, or the pair's slice of the global scratch
         // (a bin whose candidates fit the warp scratch keeps its lists there even when the global scratch exists; it is
-        // allocated whenever R * 256 > LIST_CAP_WS)
-        const bool spill = P.dlist && Ktot > LIST_CAP_WS;
-        const int LIST_CAP = spill ? R * NPOSE : LIST_CAP_WS;         // >= Ktot
-        uint16_t* list = spill ? P.dlist + (int64_t)env * 2 * (R * NPOSE) : reinterpret_cast<uint16_t*>(W_pts);
-        auto cell_of = [](int e) { const int b = e & 255; return (e >> 8) * NPOSE + (b & 15) * 16 + (b >> 4); };
+        // allocated whenever R * NPOSE > LIST_CAP_WS).  An entry is r << 2 LOG | b, b the bit of the pose in the rotation's set
+        // (b = ly * AY + lx: contour points are (column, row) = (ly, lx))
+        const bool spill = P.dlist && Ktot > CS::LIST_CAP_WS;
+        const int LIST_CAP = spill ? R * G::NPOSE : CS::LIST_CAP_WS;         // >= Ktot
+        uint16_t* list = spill ? P.dlist + (int64_t)env * 2 * (R * G::NPOSE) : reinterpret_cast<uint16_t*>(W_pts);
+        auto cell_of = [](int e) { const int b = e & (G::NPOSE - 1); return (e >> (2 * LOG)) * G::NPOSE + (b & MASK) * G::AY + (b >> LOG); };
         {
             for (int r = 0; r < R; ++r) {
-                const uint32_t* cb = cbits + r * 8;
+                const uint32_t* cb = cbits + r * G::BMW;
                 int ord0 = __shfl_sync(0xffffffffu, excl, r);
 #pragma unroll
-                for (int qd = 0; qd < 8; ++qd) {
+                for (int qd = 0; qd < G::BMW; ++qd) {
                     const uint32_t wbits = cb[qd];
                     if ((wbits >> lane) & 1u)
-                        list[ord0 + __popc(wbits & ((1u << lane) - 1u))] = (uint16_t)((r << 8) | (qd * 32 + lane));
+                        list[ord0 + __popc(wbits & ((1u << lane) - 1u))] = (uint16_t)((r << (2 * LOG)) | (qd * 32 + lane));
                     ord0 += __popc(wbits);
                 }
             }
@@ -1372,9 +1487,9 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
             if (Ktot <= sel) {
                 for (int i = lane; i < Ktot; i += 32) {
                     const int e = list[i];
-                    const int b = e & 255;
+                    const int b = e & (G::NPOSE - 1);
                     bool m; const double H = height_of(cell_of(e), m);
-                    put_row(i, e >> 8, b & 15, b >> 4, H, m ? 1.0 : 0.0);
+                    put_row(i, e >> (2 * LOG), b & MASK, b >> LOG, H, m ? 1.0 : 0.0);
                 }
             } else {
                 // More candidates than rows: keep the `sel` lowest heights, ties by original order (stable
@@ -1432,7 +1547,7 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                 for (int i0 = 0; i0 < Ktot; i0 += 32) {
                     const int i = i0 + lane;
                     const int e = i < Ktot ? list[i] : 0;
-                    const int b = e & 255;
+                    const int b = e & (G::NPOSE - 1);
                     bool m = false; double H = 0.0;
                     if (i < Ktot) H = height_of(cell_of(e), m);
                     const uint32_t inv = __ballot_sync(0xffffffffu, i < Ktot && !m);
@@ -1446,11 +1561,11 @@ __global__ void __launch_bounds__(32 * EPC, cand_min_ctas<EPC>()) irbpp_candidat
                                 const double H2 = posz_g[cell_of(e2)];
                                 rank += (H2 < H) || (H2 == H && e2 < e);
                             }
-                            if (rank < sel) put_row(rank, e >> 8, b & 15, b >> 4, H, 1.0);
+                            if (rank < sel) put_row(rank, e >> (2 * LOG), b & MASK, b >> LOG, H, 1.0);
                         }
                     } else if (i < Ktot) {
                         const int rank = nvalid + inv_before + __popc(inv & ((1u << lane) - 1u));
-                        if (rank < sel) put_row(rank, e >> 8, b & 15, b >> 4, H, 0.0);
+                        if (rank < sel) put_row(rank, e >> (2 * LOG), b & MASK, b >> LOG, H, 0.0);
                     }
                     inv_before += __popc(inv);
                 }

@@ -2,9 +2,9 @@
 //
 // The float32 observation of a bin is [sel x (rot, x, y, H, V) | next_item_vec(9) | heightmap(1024)] = 14 132 bytes at
 // sel = 500 (binPhy.py:196-227), most of it small integers stored as floats and zero padding.  Between GPUs it travels as
-//   u16 rot << 8 | x << 4 | y  per row  |  f32 H per row  |  one V bit per row  |  f32 item id  |  f32 heightmap
+//   u16 rot << 10 | x << 5 | y  per row  |  f32 H per row  |  one V bit per row  |  f32 item id  |  f32 heightmap
 // = 7 184 bytes at sel = 500 (51 %), and is expanded on the receiver.  The encoding is exact for what the environment
-// emits: rot < 256, x, y < 16 integers, V in {0, 1}, next_item_vec = (id, 0, ..., 0) (binPhy.py:191).
+// emits on either action grid: rot < 64, x, y < 32 integers, V in {0, 1}, next_item_vec = (id, 0, ..., 0) (binPhy.py:191).
 #pragma once
 #include <stdint.h>
 
@@ -28,7 +28,7 @@ __global__ void irbpp_pack_obs_kernel(const float* __restrict__ obs, int64_t obs
             const int row = 2 * i + h;
             if (row < sel) {
                 const float* r = o + row * 5;
-                w |= ((((uint32_t)r[0]) << 8) | (((uint32_t)r[1]) << 4) | ((uint32_t)r[2])) << (16 * h);
+                w |= ((((uint32_t)r[0]) << 10) | (((uint32_t)r[1]) << 5) | ((uint32_t)r[2])) << (16 * h);
             }
         }
         p[i] = w;
@@ -58,7 +58,7 @@ __global__ void irbpp_unpack_obs_kernel(const uint32_t* __restrict__ in, int sel
     for (int row = threadIdx.x; row < sel; row += blockDim.x) {
         const uint32_t c = (p[row >> 1] >> (16 * (row & 1))) & 0xFFFFu;
         float* r = o + row * 5;
-        r[0] = (float)(c >> 8); r[1] = (float)((c >> 4) & 15u); r[2] = (float)(c & 15u);
+        r[0] = (float)(c >> 10); r[1] = (float)((c >> 5) & 31u); r[2] = (float)(c & 31u);
         r[3] = hp[row];
         r[4] = ((vp[row >> 5] >> (row & 31)) & 1u) ? 1.0f : 0.0f;
     }

@@ -58,7 +58,8 @@ def _env_kwargs(args):
                 selected_action=int(getattr(args, "selectedAction", 500)),
                 buffer_size=int(getattr(args, "bufferSize", 1)),
                 bin_dimension=tuple(getattr(args, "bin_dimension", (0.32, 0.32, 0.30))),
-                resolution_act=float(getattr(args, "resolutionA", 0.02)),
+                # no args.resolutionA: the library's own (GpuVecEnv checks that the two agree)
+                resolution_act=float(args.resolutionA) if hasattr(args, "resolutionA") else None,
                 resolution_h=float(getattr(args, "resolutionH", 0.01)),
                 resolution_z=float(getattr(args, "resolutionZ", 0.01)))
 

@@ -190,10 +190,14 @@ class GpuVecEnv(VecEnv):
       over the window of ``num_trajectories`` (default: all from ``first_trajectory`` on).  ``trajectory[e]`` is the
       trajectory bin e plays (-1 before its first reset); a bin whose next trajectory lies beyond the window is
       ``idle``: zero observation rows, reward 0, done False, ``info['Valid']`` False, its actions ignored.  Both are
-      followed on the host from resets and the ``done`` flags ``step_wait`` returns."""
+      followed on the host from resets and the ``done`` flags ``step_wait`` returns.
+
+    ``resolution_act`` is the action resolution the library's windows were computed for (``library.resolutionAct``, the
+    default); another value raises ``ValueError``.  0.02 gives the 16 x 16 action grid, 0.01 (``resolutionA`` =
+    ``resolutionH``, as the reference trains the Cube dataset) the 32 x 32 grid; ``Ax``, ``Ay`` are its sizes."""
 
     def __init__(self, library, sequences, num_envs=None, device="cuda:0", selected_action=500, buffer_size=1,
-                 bin_dimension=(0.32, 0.32, 0.30), resolution_act=0.02, resolution_h=0.01, resolution_z=0.01,
+                 bin_dimension=(0.32, 0.32, 0.30), resolution_act=None, resolution_h=0.01, resolution_z=0.01,
                  approx_legacy=False, item_seed=0, item_groups=None, trajectories=None, first_trajectory=1,
                  num_trajectories=None):
         import torch
@@ -204,6 +208,15 @@ class GpuVecEnv(VecEnv):
             raise RuntimeError("GpuVecEnv needs a CUDA device; there is no CPU path")
         if sum(x is not None for x in (sequences, item_groups, trajectories)) > 1:
             raise ValueError("sequences, item_groups and trajectories are mutually exclusive")
+        if resolution_act is None:
+            resolution_act = float(library.resolutionAct)
+        elif float(resolution_act) != float(library.resolutionAct):
+            # the library's windows (rangeX_OA, rangeY_OA) were computed for its own action resolution
+            raise ValueError("resolution_act %r differs from the library's resolutionAct %r"
+                             % (resolution_act, library.resolutionAct))
+        # action grid (Space.__init__, space.py:19-24)
+        self.Ax = int(np.ceil(float(bin_dimension[0]) / resolution_act))
+        self.Ay = int(np.ceil(float(bin_dimension[1]) / resolution_act))
         if sequences is None:
             # no explicit sequences: ids are drawn on the device, i.i.d. uniform from a counter-based generator
             # seeded with ``item_seed`` (RandomItemCreator's role, IRcreator.py:26-33; no period)
@@ -507,11 +520,11 @@ class GpuVecEnv(VecEnv):
         torch = self._torch
         if isinstance(poses, torch.Tensor):
             if poses.dim() == 2:
-                poses = (poses[:, 0].to(torch.int64) * 16 + poses[:, 1].to(torch.int64)) * 16 + poses[:, 2].to(torch.int64)
+                poses = (poses[:, 0].to(torch.int64) * self.Ax + poses[:, 1].to(torch.int64)) * self.Ay + poses[:, 2].to(torch.int64)
         else:
             poses = np.asarray(poses)
             if poses.ndim == 2:
-                poses = (poses[:, 0].astype(np.int64) * 16 + poses[:, 1]) * 16 + poses[:, 2]
+                poses = (poses[:, 0].astype(np.int64) * self.Ax + poses[:, 1]) * self.Ay + poses[:, 2]
             poses = np.ascontiguousarray(poses, dtype=np.int64)
         keep, ptr, on_dev = self._actions_arg(poses, "poses")
         obs = self._take_obs()
@@ -557,7 +570,8 @@ class GpuVecEnv(VecEnv):
     def debug_scan(self, item_ids):
         n, R, sel = self.num_envs, self.library.num_rotations, self.selected_action
         items = np.ascontiguousarray(item_ids, dtype=np.int32).reshape(n)
-        pz = np.zeros((n, R, 16, 16)); pv = np.zeros((n, R, 16, 16)); mk = np.zeros((n, R, 16, 16))
+        grid = (n, R, self.Ax, self.Ay)
+        pz = np.zeros(grid); pv = np.zeros(grid); mk = np.zeros(grid)
         cand = np.zeros((n, sel, 5)); nh = np.zeros(n, np.int32)
         self._check(self._lib.irbpp_debug_scan(self._h, items.ctypes.data, pz.ctypes.data, pv.ctypes.data,
                                                mk.ctypes.data, cand.ctypes.data, nh.ctypes.data))
@@ -565,8 +579,8 @@ class GpuVecEnv(VecEnv):
 
     def debug_hulls(self, posZValid, mask):
         n, R, sel = self.num_envs, self.library.num_rotations, self.selected_action
-        pv = np.ascontiguousarray(posZValid, dtype=np.float64).reshape(n, R, 16, 16)
-        mk = np.ascontiguousarray(mask, dtype=np.float64).reshape(n, R, 16, 16)
+        pv = np.ascontiguousarray(posZValid, dtype=np.float64).reshape(n, R, self.Ax, self.Ay)
+        mk = np.ascontiguousarray(mask, dtype=np.float64).reshape(n, R, self.Ax, self.Ay)
         cand = np.zeros((n, sel, 5)); nh = np.zeros(n, np.int32)
         self._check(self._lib.irbpp_debug_hulls(self._h, pv.ctypes.data, mk.ctypes.data, cand.ctypes.data,
                                                 nh.ctypes.data))
