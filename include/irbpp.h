@@ -317,6 +317,41 @@ int irbpp_replay_sample(const irbpp_replay_memory* mem, const int32_t* mem_ids, 
 int irbpp_replay_update_priorities(const irbpp_replay_memory* mem, const int32_t* mem_ids, const int64_t* tree_idxs,
                                    const float* loss, int32_t B, double omega, uint32_t* error_flags, void* stream);
 
+/* ---- the location network's forward pass and Agent.act (csrc/irbpp_actor.cuh) ----------------------------------------
+ * DQNBPP.forward with bufferSize == 1 (model.py:316-352, 386-404) followed by Agent.act (agent.py:51-58), for N bins at
+ * once.  Handle-free: every pointer is device memory owned by the caller, all on one device; errors are reported
+ * through irbpp_last_error(NULL).  Weights are float32, contiguous, in nn.Conv2d / nn.Linear layouts (out x in); the
+ * NoisyLinear layers take the EFFECTIVE weights of the mode the network acts in (train: mu + sigma * epsilon; eval: mu).
+ * Supported: hidden_size 128, 1 <= atoms <= 32, selected_action >= 1, the 32 x 32 heightmap. */
+typedef struct {
+    const float* conv1_w; const float* conv1_b;     /* heightEncoder.conv1 [16, 1, 4, 4], [16] */
+    const float* conv2_w; const float* conv2_b;     /* heightEncoder.conv2 [32, 16, 4, 4], [32] */
+    const float* conv3_w; const float* conv3_b;     /* heightEncoder.conv3 [4, 32, 3, 3], [4] */
+    const float* cand1_w; const float* cand1_b;     /* init_candidate_embed.0 [32, 4], [32] */
+    const float* cand2_w; const float* cand2_b;     /* init_candidate_embed.2 [128, 32], [128] */
+    const float* proj1_w; const float* proj1_b;     /* project_layer.0 [256, 512], [256] */
+    const float* proj2_w; const float* proj2_b;     /* project_layer.2 [128, 256], [128] */
+    const float* fc_h_v_w; const float* fc_h_v_b;   /* fc_h_v [128, 128], [128] */
+    const float* fc_z_v_w; const float* fc_z_v_b;   /* fc_z_v [atoms, 128], [atoms] */
+    const float* fc_h_a_w; const float* fc_h_a_b;   /* fc_h_a [128, 128], [128] */
+    const float* fc_z_a_w; const float* fc_z_a_b;   /* fc_z_a [atoms, 128], [atoms] */
+    float negative_slope;                           /* of every LeakyReLU (nn.LeakyReLU default 0.01) */
+} irbpp_dqn_weights;
+
+/* Bytes of the scratch irbpp_dqn_act needs for N bins of selected_action rows (-1 for bad sizes). */
+int64_t irbpp_dqn_scratch_bytes(int32_t N, int32_t selected_action);
+
+/* obs float32 [N] rows of obs_stride >= selected_action * 5 + 9 + 1024 (model.py:174-182: candidate rows
+ * [rot, x, y, H, mask], the next item, the 32 x 32 heightmap); shape_feature float32 [N, 128]; support float32 [atoms].
+ * mask: float32 at mask[b * mask_row_stride + r * mask_elem_stride] (the strided view get_mask_from_state returns has
+ * element stride 5), or NULL for no masking.  Writes actions int64 [N] (argmax over the rows of the masked expected
+ * value, first index on ties, 0 for a fully masked bin) and, when sum_q_map is not NULL, the masked expected values
+ * float32 [N, selected_action] (-inf where mask != 1).  scratch: irbpp_dqn_scratch_bytes bytes, 256-byte aligned. */
+int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t selected_action,
+                  const float* shape_feature, const float* support, int32_t atoms, const float* mask, int64_t mask_row_stride,
+                  int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch, int64_t scratch_bytes,
+                  void* stream);
+
 /* Profiling aid: when enabled, thread 0 of every CTA adds the SM cycles it spent in each kernel phase
  * (0 scan kernel: load + apply action, 1 scan kernel: observation heightmap + scan + level bitmaps,
  * 2 candidates kernel: contour tasks, 3 candidates kernel: select / pad) to counters 0-3; counters 4-7 count

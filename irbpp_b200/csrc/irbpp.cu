@@ -22,6 +22,7 @@
 #include "irbpp_pointnet.cuh"
 #include "irbpp_pack.cuh"
 #include "irbpp_replay.cuh"
+#include "irbpp_actor.cuh"
 
 using namespace irbpp;
 
@@ -1056,6 +1057,50 @@ int irbpp_replay_update_priorities(const irbpp_replay_memory* mem, const int32_t
     DeviceGuard guard(device_of(mem->tree));
     const int blocks = (mem->num_memories + RP_UPDATE_WARPS - 1) / RP_UPDATE_WARPS;
     irbpp_replay_update_kernel<<<blocks, 32 * RP_UPDATE_WARPS, 0, (cudaStream_t)stream>>>(A);
+    return launch_status();
+}
+
+// ---- the location network's forward pass and Agent.act (csrc/irbpp_actor.cuh) -------------------------------------
+int64_t irbpp_dqn_scratch_bytes(int32_t N, int32_t selected_action) {
+    if (N <= 0 || selected_action <= 0) return -1;
+    return actor_scratch_bytes(N, selected_action);
+}
+
+int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t selected_action,
+                  const float* shape_feature, const float* support, int32_t atoms, const float* mask, int64_t mask_row_stride,
+                  int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch, int64_t scratch_bytes,
+                  void* stream) {
+    if (!weights || !obs || !shape_feature || !support || !actions || !scratch) return fail(nullptr, IRBPP_EINVAL, "null act argument");
+    if (N <= 0 || selected_action <= 0) return fail(nullptr, IRBPP_EINVAL, "need N >= 1 bins and selected_action >= 1 (N %d, sel %d)", N, selected_action);
+    if (atoms < 1 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [1, %d]", atoms, AC_MAXATOMS);
+    if (obs_stride < (int64_t)selected_action * 5 + 9 + AC_HM * AC_HM)
+        return fail(nullptr, IRBPP_EINVAL, "observation stride %lld < selected_action * 5 + 9 + 1024", (long long)obs_stride);
+    if (scratch_bytes < actor_scratch_bytes(N, selected_action))
+        return fail(nullptr, IRBPP_EINVAL, "scratch of %lld bytes < %lld", (long long)scratch_bytes, (long long)actor_scratch_bytes(N, selected_action));
+    if (reinterpret_cast<uintptr_t>(scratch) & 255) return fail(nullptr, IRBPP_EINVAL, "scratch not 256-byte aligned");
+    const irbpp_dqn_weights& w = *weights;
+    const float* ptrs[] = {w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.cand1_w, w.cand1_b, w.cand2_w,
+                           w.cand2_b, w.proj1_w, w.proj1_b, w.proj2_w, w.proj2_b, w.fc_h_v_w, w.fc_h_v_b, w.fc_z_v_w,
+                           w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b};
+    for (const float* p : ptrs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null weight pointer");
+    ActorParams A;
+    memset(&A, 0, sizeof(A));
+    A.w = ActorWeights{w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.cand1_w, w.cand1_b, w.cand2_w,
+                       w.cand2_b, w.proj1_w, w.proj1_b, w.proj2_w, w.proj2_b, w.fc_h_v_w, w.fc_h_v_b, w.fc_z_v_w,
+                       w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b, w.negative_slope};
+    A.obs = obs; A.obs_stride = obs_stride; A.N = N; A.sel = selected_action; A.atoms = atoms;
+    A.shape_feature = shape_feature; A.support = support;
+    A.mask = mask; A.mask_row = mask_row_stride; A.mask_elem = mask_elem_stride;
+    A.actions = actions; A.sum_q = sum_q_map;
+    actor_scratch_layout(A, scratch);
+    const int dev = device_of(obs);
+    DeviceGuard guard(dev);
+    cudaError_t e = raise_dynamic_smem(dev, (const void*)irbpp_actor_rows_kernel, AC_ROWS_SMEM_BYTES);
+    if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "rows kernel set-up: %s", cudaGetErrorString(e));
+    cudaStream_t s = (cudaStream_t)stream;
+    irbpp_actor_bin_kernel<<<N, AC_THREADS, 0, s>>>(A);
+    irbpp_actor_rows_kernel<<<N, AC_THREADS, AC_ROWS_SMEM_BYTES, s>>>(A);
     return launch_status();
 }
 
