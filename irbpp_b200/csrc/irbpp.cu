@@ -565,7 +565,7 @@ int irbpp_set_trajectories(irbpp_handle h, const int32_t* items, const int64_t* 
     const int64_t M = offsets[num_trajectories];
     for (int64_t i = 0; i < M; ++i)
         if (items[i] < 0 || items[i] >= h->P.S) return fail(h, IRBPP_EINVAL, "item id %d out of range at %lld", items[i], (long long)i);
-    const int nfill = h->P.K > 1 ? h->P.K : 1;       // what reset() previews
+    const int nfill = queue_len(h->P.K);             // what reset() previews
     for (int t = first; t < first + count; ++t)
         if (offsets[t + 1] - offsets[t] < nfill)
             return fail(h, IRBPP_EINVAL, "trajectory %d has %lld items, a reset takes %d", t, (long long)(offsets[t + 1] - offsets[t]), nfill);
@@ -809,7 +809,7 @@ int irbpp_debug_state(irbpp_handle h, double* heightmap, int32_t* queue, int32_t
     if (queue || cursor || packed_count) {
         std::vector<EnvState> st((size_t)N);
         CUDA_TRY(h, cudaMemcpy(st.data(), h->P.state, st.size() * sizeof(EnvState), cudaMemcpyDeviceToHost));
-        const int k = h->P.K > 1 ? h->P.K : 1;
+        const int k = queue_len(h->P.K);
         for (int e = 0; e < N; ++e) {
             if (queue) for (int i = 0; i < k; ++i) queue[(size_t)e * k + i] = st[e].queue[i];
             if (cursor) cursor[e] = st[e].cursor;

@@ -59,7 +59,17 @@ struct Grid {
     static constexpr int BMW = NPOSE / 32;                     // words of a pose bit set (feasibility, level image, candidates)
     using Img = ImageGrid<LOG>;
     static_assert((STEP_ == 1 || STEP_ == 2) && AX == AY && AY == (1 << LOG), "supported action grids: 16x16 and 32x32");
-    __host__ __device__ static int pack(int rot, int x, int y) { return (rot << (2 * LOG)) | (x << LOG) | y; }
+    __host__ __device__ __forceinline__ static int pack(int rot, int x, int y) { return (rot << (2 * LOG)) | (x << LOG) | y; }
+    template <class T> __host__ __device__ __forceinline__ static T rot_of(T p) { return p >> (2 * LOG); }   // T: the entry's own type
+    template <class T> __host__ __device__ __forceinline__ static T x_of(T p) { return (p >> LOG) & MASK; }
+    template <class T> __host__ __device__ __forceinline__ static T y_of(T p) { return p & MASK; }
+    // A phase D list entry rot << 2 LOG | b -> the pose and its flat index.  b is the pose's bit in the rotation's candidate
+    // set, which is indexed by contour point (column, row) = (ly, lx): b = ly * AY + lx, x and y transposed against pack.
+    struct ListPose { int rot, x, y, cell; };
+    __host__ __device__ __forceinline__ static ListPose list_pose(int e) {
+        const int rot = rot_of(e), b = e & (NPOSE - 1), x = b & MASK, y = b >> LOG;
+        return {rot, x, y, rot * NPOSE + x * AY + y};
+    }
 };
 constexpr int CTA_THREADS = 128;
 constexpr int CTA_WARPS = CTA_THREADS / 32;
@@ -240,6 +250,11 @@ __device__ __forceinline__ void store_error(const Params& P, int env, int err) {
 // cell (x, y) of a bin's heightmap in the column-parity planes: [y & 1][x][y >> 1]
 __host__ __device__ __forceinline__ int hm_index(int x, int y) { return ((y & 1) * HX + x) * (HY / 2) + (y >> 1); }
 
+// all threads of a CTA: zero one bin's heightmap (8 KB, shared or global memory) with 16-byte stores
+__device__ __forceinline__ void zero_heightmap(double* hm) {
+    for (int i = threadIdx.x; i < HX * HY / 2; i += CTA_THREADS) reinterpret_cast<double2*>(hm)[i] = make_double2(0.0, 0.0);
+}
+
 // splitmix64 of (seed, env, draw counter): the 64-bit value behind the counter-based item sources
 __host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint32_t env, uint32_t counter) {
     uint64_t z = seed + 0x9E3779B97F4A7C15ull * (((uint64_t)env << 32) | counter) + 0x9E3779B97F4A7C15ull;
@@ -310,6 +325,9 @@ __device__ __forceinline__ bool begin_trajectory(const Params& P, EnvState& st, 
 __device__ __forceinline__ bool env_idle(const Params& P, int env) {
     return P.item_src == ITEMS_TRAJ && P.state[env].traj_len == TRAJ_IDLE;
 }
+
+// items in a bin's queue, what reset() fills: buffer_size, one for the online setting (K = 1)
+__host__ __device__ __forceinline__ int queue_len(int K) { return K > 1 ? K : 1; }
 
 __host__ __device__ __forceinline__ bool mode_emits_loc(int mode, int K) {
     return !((mode == MODE_STEP || mode == MODE_RESET) && K > 1);
@@ -405,6 +423,16 @@ __device__ __forceinline__ int level_of(const Params& P, double posz, double inv
 }
 
 // ---- phase B: one warp scans one rotation -------------------------------------------------------------
+// The scan list of a rotation, staged in this warp's shared-memory buffer `es` between two warp barriers (all lanes then
+// read the same entry: a broadcast); `also` runs between the same barriers.
+template <class F>
+__device__ __forceinline__ void stage_scan_list(const Params& P, const ShapeRot* sr, int nt, TileEntry* es, int lane, F&& also) {
+    const TileEntry* __restrict__ te = P.tiles + sr->tile_off;
+    __syncwarp();                                   // previous rotation's readers are done
+    for (int k = lane; k < nt; k += 32) es[k] = te[k];
+    also();
+    __syncwarp();
+}
 // Block form, stepSize 2 only (the blocks are aligned to the 2x2 / 4x4 action windows).
 // Writes posz[r][256], maskbits[r][8], the level bitmaps and their count (space.py:98-129,
 // cvTools.py:78-85).  Returns true if any pose is feasible.
@@ -419,12 +447,7 @@ __device__ __forceinline__ bool scan_rotation(const Params& P, const double* arr
     const int nX = sr->nX, nY = sr->nY, nt = sr->ntiles;
     const double ez = sr->ez;
     const double init = sr->any_zero ? 0.0 : -INFINITY;
-    {
-        const TileEntry* __restrict__ te = P.tiles + sr->tile_off;
-        __syncwarp();                                   // previous rotation's readers are done
-        for (int k = lane; k < nt; k += 32) es[k] = te[k];
-        __syncwarp();
-    }
+    stage_scan_list(P, sr, nt, es, lane, [] {});
     const double inv = 1.0 / P.resZ;
     double* posz_g = posz_of<G>(P, env, r);
     uint32_t* mask_g = maskbits_of<G>(P, env, r);
@@ -487,16 +510,10 @@ __device__ __forceinline__ bool scan_rotation_dense(const Params& P, const doubl
     const int V = nX * nY;
     const double ez = sr->ez;
     const double init = sr->any_zero ? 0.0 : -INFINITY;
-    {
-        const TileEntry* __restrict__ te = P.tiles + sr->tile_off;
-        __syncwarp();                                   // previous rotation's readers are done
-        for (int k = lane; k < nt; k += 32) es[k] = te[k];
-        reinterpret_cast<uint32_t*>(lv_s)[lane] = 0u;
-        reinterpret_cast<uint32_t*>(lv_s)[lane + 32] = 0u;
+    stage_scan_list(P, sr, nt, es, lane, [&] {                 // and clear the level map
 #pragma unroll
-        for (int q = 2; q < G::NPOSE / 128; ++q) reinterpret_cast<uint32_t*>(lv_s)[lane + 32 * q] = 0u;
-        __syncwarp();
-    }
+        for (int q = 0; q < G::NPOSE / 128; ++q) reinterpret_cast<uint32_t*>(lv_s)[lane + 32 * q] = 0u;
+    });
     const double inv = 1.0 / P.resZ;
     double* posz_g = posz_of<G>(P, env, r);
     // v / nY == (v * magic) >> 16 whenever v * nY < 2^16: v < NPOSE, nY <= AY (256 * 16 and 1024 * 32 are both below 2^16)
@@ -622,7 +639,7 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
     __shared__ double M_s[NBLK];                         // block maxima of the heightmap (block form of phase B)
     __shared__ double P2_s[NBLK];                        // 2x2 block maxima
     __shared__ double z_sh;
-    __shared__ int ok_sh, rot_sh, lx_sh, ly_sh, item_sh, err_sh, any_sh;   // item_sh < 0: the bin is idle (no trajectory left)
+    __shared__ int ok_sh, item_sh, err_sh, any_sh;   // item_sh < 0: the bin is idle (no trajectory left)
     __shared__ __align__(8) mbarrier_t mbar;             // completion of the bulk copies of this bin's inputs
     __shared__ __align__(16) ShapeRot srot_s[MAX_ROT];   // (56 bytes each) table headers of the item the action places (all rotations), prefetched
     __shared__ long long a_sh;                           // the bin's action
@@ -668,10 +685,7 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
         reinterpret_cast<uint32_t*>(&st_s)[lane] = stw;
         if (mode == MODE_STEP && lane == 0) a_sh = a_pf;
     }
-    if (mode == MODE_RESET) {
-        double2* dst = reinterpret_cast<double2*>(hm_s);
-        for (int i = tid; i < HX * HY / 2; i += CTA_THREADS) dst[i] = make_double2(0.0, 0.0);
-    }
+    if (mode == MODE_RESET) zero_heightmap(hm_s);
     if (tid == 0) { err_sh = 0; any_sh = 0; }
     __syncthreads();                       // mbarrier initialised, state in shared memory
     // trajectory replay: a bin with no trajectory left ignores every call (no draw, no placement, no error)
@@ -697,12 +711,13 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
     int next_seq = st_s.next_seq;          // thread 0's register copy; written back with the state
     int draw_err = 0;                      // thread 0: ERR_TRAJ_END of a draw past the trajectory's end
     auto draw = [&]() { return draw_item<TRAJ>(P, env, st_s, next_seq, draw_err); };
-    // thread 0, reset / auto-reset: the next trajectory; false when the bin turns idle
-    auto new_episode = [&]() { return !TRAJ || begin_trajectory(P, st_s, next_seq, tb_pf, te_pf); };
-    // zero the bin's heightmap in global memory (reset / auto-reset); the shared copy is zeroed by the caller
-    auto zero_hm_global = [&]() {
-        double2* dst = reinterpret_cast<double2*>(hm_g);
-        for (int i = tid; i < HX * HY / 2; i += CTA_THREADS) dst[i] = make_double2(0.0, 0.0);
+    // thread 0, reset and auto-reset (reset(), binPhy.py): clear the episode counters, start the next trajectory and fill
+    // the queue; false when the bin has no trajectory left (it turns idle)
+    auto start_episode = [&]() {
+        st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0; st_s.order_act = 0;
+        const bool live = !TRAJ || begin_trajectory(P, st_s, next_seq, tb_pf, te_pf);
+        if (live) for (int q = 0; q < queue_len(P.K); ++q) queue_g[q] = draw();
+        return live;
     };
 
     // ---- phase A: bookkeeping / apply action ----
@@ -712,25 +727,17 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
             if (mode == MODE_STEP)         // reward 0, done 0, Valid 0: trainer-style loops skip the bin
                 store_results(P, env, 0.0f, 0, 0, -1, 0, -1.0, 0.0);
         }
-        __syncthreads();
     } else if (mode == MODE_RESET) {
         if (tid == 0) {
-            const int nfill = P.K > 1 ? P.K : 1;
-            const bool live = new_episode();
-            if (live)
-                for (int q = 0; q < nfill; ++q) queue_g[q] = draw();
+            const bool live = start_episode();
             if (draw_err) err_sh = draw_err;
-            st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0;
-            st_s.order_act = 0;
             item_sh = live ? queue_g[0] : -1;
         }
-        zero_hm_global();
-        __syncthreads();
+        zero_heightmap(hm_g);              // the shared copy was zeroed during the loads
     } else if (mode == MODE_STEP) {
         // every thread decodes the action: the whole CTA then fetches the placed rotation's top table (what the
         // heightmap update needs) while warp 0 computes the drop height of that single pose from the bottom table --
         // the two table reads overlap instead of following each other
-        const int item = st_s.cur_item;
         int rot = 0, lx = 0, ly = 0;
         bool ok = true;
         {
@@ -738,7 +745,7 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
             if (a < 0 || a >= (P.pose_actions ? P.R * G::NPOSE : P.sel)) { ok = false; if (tid == 0) err_sh = 2; }
             else {
                 const uint32_t c = P.pose_actions ? (uint32_t)a : (uint32_t)cand_s[a];
-                rot = c >> (2 * G::LOG); lx = (c >> G::LOG) & G::MASK; ly = c & G::MASK;
+                rot = G::rot_of(c); lx = G::x_of(c); ly = G::y_of(c);
                 if (rot >= P.R) { rot = 0; ok = false; if (tid == 0) err_sh = 2; }
             }
         }
@@ -788,11 +795,10 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
                 if (v > hm_s[idx]) { hm_s[idx] = v; hm_g[idx] = v; }
             }
         } else {
-            for (int i = tid; i < HX * HY; i += CTA_THREADS) hm_s[i] = 0.0;    // auto-reset
-            zero_hm_global();
+            zero_heightmap(hm_s); zero_heightmap(hm_g);       // auto-reset
         }
         if (tid == 0) {
-            const int nfill = P.K > 1 ? P.K : 1;
+            const int nfill = queue_len(P.K);
             bool live = true;
             if (ok) {
                 const double rew = rew_pf;
@@ -806,16 +812,11 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
                 queue_g[nfill - 1] = draw();
             } else {
                 store_results(P, env, 0.0f, 1, 1, st_s.packed, st_s.ep_len + 1, st_s.vol_sum / P.binvol, st_s.ep_rew + 0.0);
-                st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0;
-                st_s.order_act = 0;
-                live = new_episode();
-                if (live)
-                    for (int q = 0; q < nfill; ++q) queue_g[q] = draw();   // reset(): clear + preview
+                live = start_episode();
             }
             if (draw_err) err_sh = draw_err;
             item_sh = live ? queue_g[0] : -1;
         }
-        __syncthreads();
     } else if (mode == MODE_CANDIDATES) {
         if (tid == 0) {
             int64_t oa = P.actions[env];
@@ -823,14 +824,12 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
             st_s.order_act = (int)oa;
             item_sh = queue_g[oa];
         }
-        __syncthreads();
     } else if (mode == MODE_ALL_OBS) {
         if (tid == 0) item_sh = queue_g[slot];
-        __syncthreads();
     } else {   // MODE_DEBUG_SCAN
         if (tid == 0) item_sh = P.dbg_items[env];
-        __syncthreads();
     }
+    __syncthreads();                       // item_sh, err_sh and the heightmap are final
     clock.mark(0);   // load + phase A
 
     const bool emit_loc = mode_emits_loc(mode, P.K);
@@ -985,7 +984,7 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
     double best = INFINITY;
     int beste = 0x7fffffff;
     for (int e = tid; e < P.R * G::NPOSE; e += CTA_THREADS) {
-        const int r = e >> (2 * G::LOG), p = e & (G::NPOSE - 1);
+        const int r = G::rot_of(e), p = e & (G::NPOSE - 1);
         const bool feas = (maskbits_of<G>(P, env, r)[p >> 5] >> (p & 31)) & 1u;
         double s = HEUR_INVALID;
         if (feas) {
@@ -1017,9 +1016,9 @@ __global__ void __launch_bounds__(CTA_THREADS) irbpp_heuristic_kernel(const Para
     if (first != 0x7fffffff) atomicMin(&idx_sh, first);
     __syncthreads();
     if (tid == 0) {
-        P.heur_pose[env * 3 + 0] = beste >> (2 * G::LOG);
-        P.heur_pose[env * 3 + 1] = (beste >> G::LOG) & G::MASK;
-        P.heur_pose[env * 3 + 2] = beste & G::MASK;
+        P.heur_pose[env * 3 + 0] = G::rot_of(beste);
+        P.heur_pose[env * 3 + 1] = G::x_of(beste);
+        P.heur_pose[env * 3 + 2] = G::y_of(beste);
         P.heur_index[env] = (idx_sh == 0x7fffffff) ? -1 : idx_sh;
     }
 }
@@ -1065,7 +1064,7 @@ struct CandSmem {
     static constexpr int ENVS_PER_CTA = EPC, CAND_WARPS = EPC, CAND_THREADS = 32 * EPC;
     using TaskEntry = typename std::conditional<G::LOG == 4, uint16_t, uint32_t>::type;
     uint32_t slots[CAND_THREADS * G::Img::ROWS_WORDS];    // level images of this round in padded row form (one per thread)
-    TaskEntry task_tab[TASK_TAB];                         // micro-task m < TASK_TAB: slot << 2 LOG | x << LOG | y of its start pixel
+    TaskEntry task_tab[TASK_TAB];                         // micro-task m < TASK_TAB: G::pack(slot, x, y) of its start pixel
     int32_t pre[ENVS_PER_CTA * MAX_ROT + 1];              // prefix of level counts over (bin, rotation)
     int32_t cand_off[CAND_THREADS + 1];                   // prefix of start-candidate counts over the images, in cost order
     uint16_t slot_of[CAND_THREADS];                       // image slot at each position of the cost order
@@ -1101,13 +1100,26 @@ constexpr bool cand_smem_fits() {
 static_assert(cand_smem_fits<Grid<2>>(), "16x16 grid: narrow CTAs at their largest and wide CTAs at their smallest rotation count must fit 32 warps per SM");
 static_assert(cand_smem_fits<Grid<1>>(), "32x32 grid: narrow CTAs at their largest and wide CTAs at their smallest rotation count must fit 16 warps per SM");
 
+// the largest lo in [0, n) with a[lo] <= t, for a non-decreasing a[0 .. n) with a[0] <= t
+__device__ __forceinline__ int search_le(const int32_t* a, int n, int t) {
+    int lo = 0, hi = n;
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (a[mid] <= t) lo = mid; else hi = mid; }
+    return lo;
+}
+// contour point (ex, ey) = (ly, lx) of a kept hull vertex: set its bit in the rotation's NPOSE-bit candidate set `cb`
+template <class G>
+__device__ __forceinline__ void set_candidate(uint32_t* cb, int ex, int ey) {
+    const int b = ex * G::AY + ey;
+    atomicOr(cb + (b >> 5), 1u << (b & 31));
+}
+
 template <int EPC, class G, bool TRAJ>      // G, TRAJ: as in irbpp_scan_kernel
 __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_candidates_kernel(const Params P) {
     constexpr int ENVS_PER_CTA = EPC, CAND_WARPS = EPC, CAND_THREADS = 32 * EPC;     // one warp per bin
     using CS = CandScratch<G>;
     using Img = typename G::Img;
     using Point = typename Img::Point;
-    constexpr int WS_BYTES = CS::WS_BYTES, ROWS_WORDS = Img::ROWS_WORDS, LOG = G::LOG, MASK = G::MASK;
+    constexpr int WS_BYTES = CS::WS_BYTES, ROWS_WORDS = Img::ROWS_WORDS, LOG = G::LOG;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     CandSmem<EPC, G>& S = *reinterpret_cast<CandSmem<EPC, G>*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1186,19 +1198,18 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
         __syncthreads();
         if (tid < nround) {
             const int t = base + tid;
-            int lo = 0, hi = npairs;                        // pre[lo] <= t < pre[hi]
-            while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (S.pre[mid] <= t) lo = mid; else hi = mid; }
+            const int lo = search_le(S.pre, npairs, t);     // image t is level t - pre[lo] of pair lo
             const uint4* src = reinterpret_cast<const uint4*>(bitmaps_of<G>(P, env0, 0) + ((int64_t)lo * MAX_LEVELS + (t - S.pre[lo])) * G::BMW);
+            uint32_t* rows = S.slots + tid * ROWS_WORDS;
+            S.pair_of[tid] = (uint16_t)lo;
+            uint32_t up = 0;
+            int key = 0;
             if constexpr (LOG == 4) {
                 const uint4 a = src[0], b = src[1];
-                uint32_t* rows = S.slots + tid * ROWS_WORDS;
-                S.pair_of[tid] = (uint16_t)lo;
                 const uint32_t wv[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
                 rows[0] = 0u; rows[17] = 0u;
 #pragma unroll
                 for (int k = 0; k < 8; ++k) { rows[1 + 2 * k] = (wv[k] & 0xFFFFu) << 1; rows[2 + 2 * k] = (wv[k] >> 16) << 1; }
-                uint32_t up = 0;
-                int key = 0;
 #pragma unroll
                 for (int k = 0; k < 8; ++k) {
                     const uint32_t r0 = wv[k] & 0xFFFFu, r1 = wv[k] >> 16;
@@ -1207,14 +1218,9 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                     key += __popc(r0 ^ (r0 << 1)) + __popc(r1 ^ (r1 << 1)) + __popc(r0 ^ up) + __popc(r1 ^ r0);
                     up = r1;
                 }
-                bucket = 63 - min(63, key >> 2);            // bucket 0 = longest borders
             } else {
                 // one 32-pixel row per word; the start masks are taken again from the rows when the table is filled
-                uint32_t* rows = S.slots + tid * ROWS_WORDS;
-                S.pair_of[tid] = (uint16_t)lo;
                 rows[0] = 0u; rows[33] = 0u;
-                uint32_t up = 0;
-                int key = 0;
 #pragma unroll 2
                 for (int k = 0; k < 8; ++k) {
                     const uint4 a = src[k];
@@ -1228,8 +1234,8 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                         up = r0;
                     }
                 }
-                bucket = 63 - min(63, key >> 2);
             }
+            bucket = 63 - min(63, key >> 2);                // bucket 0 = longest borders
             my_off = atomicAdd(&S.hist[bucket], 1);
         }
         __syncthreads();
@@ -1266,7 +1272,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                     while (c && off < TASK_TAB) {
                         const int b = __ffs((int)c) - 1;           // bit b: column b & 15 of row 2k + (b >> 4)
                         c &= c - 1;
-                        S.task_tab[off++] = (uint16_t)((tid << 8) | ((b & 15) << 4) | (2 * k + (b >> 4)));
+                        S.task_tab[off++] = (uint16_t)G::pack(tid, b & 15, 2 * k + (b >> 4));
                     }
                 }
             } else {
@@ -1276,7 +1282,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                     while (c && off < TASK_TAB) {
                         const int x = __ffs((int)c) - 1;
                         c &= c - 1;
-                        S.task_tab[off++] = (uint32_t)((tid << (2 * LOG)) | (x << LOG) | y);
+                        S.task_tab[off++] = (uint32_t)G::pack(tid, x, y);
                     }
                 }
             }
@@ -1291,13 +1297,13 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
         //    serves up to 32 * EPC * TASKS_PER_LANE tasks -- a 4-bin CTA of the bench workload has ~170
         constexpr int TPL = TASKS_PER_LANE;
         constexpr int BATCH = CAND_THREADS * TPL;
-        auto slot_scratch = [&](int owner) {               // point buffer of task slot `owner` (j * CAND_THREADS + thread)
+        auto slot_scratch = [&](int owner) {               // contour scratch of task slot `owner` (j * CAND_THREADS + thread)
             const int jj = owner / CAND_THREADS, th = owner - jj * CAND_THREADS;
-            return reinterpret_cast<Point*>(ws_base + (size_t)(th >> 5) * WS_BYTES +
-                                            (jj == 0 ? 0 : (FAST_CAP * 32 + (jj - 1) * CS::SLOT_CAP * 32) * CS::PT_BYTES)) + (th & 31);
+            return StridedScratch<32, FAST_CAP, LOG>{reinterpret_cast<Point*>(ws_base + (size_t)(th >> 5) * WS_BYTES +
+                (jj == 0 ? 0 : (FAST_CAP * 32 + (jj - 1) * CS::SLOT_CAP * 32) * CS::PT_BYTES)) + (th & 31), 0};
         };
         for (int mb = 0; mb < ntask; mb += BATCH) {
-            int tk[TPL];                                    // slot << 2 LOG | x << LOG | y of my tasks, -1: none
+            int tk[TPL];                                    // G::pack(slot, x, y) of my tasks, -1: none
             int npts_j[TPL];
             uint32_t ovf_bits = 0;
 #pragma unroll
@@ -1307,10 +1313,9 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                 int slot = 0, x = 0, y = 0;
                 if (has && m < TASK_TAB) {
                     const int t = S.task_tab[m];
-                    slot = t >> (2 * LOG); x = (t >> LOG) & MASK; y = t & MASK;
+                    slot = G::rot_of(t); x = G::x_of(t); y = G::y_of(t);
                 } else if (has) {                               // beyond the table: search the prefix and the image
-                    int lo = 0, hi = CAND_THREADS;              // cand_off[lo] <= m < cand_off[hi]
-                    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (S.cand_off[mid] <= m) lo = mid; else hi = mid; }
+                    const int lo = search_le(S.cand_off, CAND_THREADS, m);     // task m is start pixel m - cand_off[lo] of image lo
                     slot = S.slot_of[lo];
                     int k = m - S.cand_off[lo];
                     const uint32_t* ri = S.slots + slot * ROWS_WORDS;
@@ -1321,13 +1326,11 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                         k -= pc;
                     }
                 }
-                tk[jt] = has ? ((slot << (2 * LOG)) | (x << LOG) | y) : -1;
+                tk[jt] = has ? G::pack(slot, x, y) : -1;
                 // (a) the lane follows the border; the points stay in the task slot's scratch
                 int n = -2, area2 = 1;
                 if (has) {
-                    StridedScratch<32, FAST_CAP, LOG> sc;
-                    sc.b = slot_scratch(jt * CAND_THREADS + tid);
-                    sc.kept = 0;
+                    auto sc = slot_scratch(jt * CAND_THREADS + tid);
                     n = follow_outer_rows(sc, S.slots + slot * ROWS_WORDS, x, y, area2, jt == 0 ? FAST_CAP : CS::SLOT_CAP);
                 }
                 const bool keep = has && n != -2 && area2 <= 0;        // a raster-first start of an outer border
@@ -1343,7 +1346,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
             for (int jt = 0; jt < TPL; ++jt) {
                 boff[jt] = atomicAdd(&S.hist[63 - min(63, npts_j[jt])], 1);
                 S.n_of[jt * CAND_THREADS + tid] = (uint8_t)npts_j[jt];
-                S.q_of[jt * CAND_THREADS + tid] = (uint16_t)(tk[jt] >= 0 ? S.pair_of[tk[jt] >> (2 * LOG)] : 0);
+                S.q_of[jt * CAND_THREADS + tid] = (uint16_t)(tk[jt] >= 0 ? S.pair_of[G::rot_of(tk[jt])] : 0);
             }
             __syncthreads();
             if (warp == 0) bucket_prefix64(S.hist, S.hbase, lane);
@@ -1358,12 +1361,9 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                 const int owner = S.order2[jt * CAND_THREADS + tid];
                 const int on = S.n_of[owner];
                 if (on > 0) {
-                    StridedScratch<32, FAST_CAP, LOG> sc;
-                    sc.b = slot_scratch(owner);
-                    sc.kept = 0;
+                    auto sc = slot_scratch(owner);
                     uint32_t* cb = candbits + (int)S.q_of[owner] * G::BMW;
-                    approx_and_emit(sc, on, P.legacy != 0,
-                                    [&](int ex, int ey) { const int b = ex * G::AY + ey; atomicOr(cb + (b >> 5), 1u << (b & 31)); });
+                    approx_and_emit(sc, on, P.legacy != 0, [&](int ex, int ey) { set_candidate<G>(cb, ex, ey); });
                 }
             }
             __syncthreads();           // scratch of every lane is free again
@@ -1380,10 +1380,10 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                         typename CS::Big bs;
                         if constexpr (CS::OVF_GLOBAL) bs.b = P.ovf + ((int64_t)blockIdx.x * EPC + warp) * CS::OVF_BYTES;
                         else bs.b = W_pts;
-                        const int slot = tk[jt] >> (2 * LOG), q = S.pair_of[slot];
+                        const int slot = G::rot_of(tk[jt]), q = S.pair_of[slot];
                         uint32_t* cb = candbits + q * G::BMW;
-                        if (!process_start_candidate(bs, S.slots + slot * ROWS_WORDS, (tk[jt] >> LOG) & MASK, tk[jt] & MASK, P.legacy != 0,
-                                [&](int ex, int ey) { const int b = ex * G::AY + ey; atomicOr(cb + (b >> 5), 1u << (b & 31)); }))
+                        if (!process_start_candidate(bs, S.slots + slot * ROWS_WORDS, G::x_of(tk[jt]), G::y_of(tk[jt]), P.legacy != 0,
+                                                     [&](int ex, int ey) { set_candidate<G>(cb, ex, ey); }))
                             atomicMax(&S.error[q / R], 6);
                     }
                     __syncwarp();
@@ -1445,7 +1445,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
         const int total = R * G::NPOSE;
         if (!anym) {
             const int nrow = total < sel ? total : sel;
-            for (int i = lane; i < nrow; i += 32) put_row(i, i >> (2 * LOG), (i >> LOG) & MASK, i & MASK, P.binz, 0.0);
+            for (int i = lane; i < nrow; i += 32) put_row(i, G::rot_of(i), G::x_of(i), G::y_of(i), P.binz, 0.0);
             zero_rows(nrow);
         } else {
             for (int i = lane; i < total; i += 32) {
@@ -1455,7 +1455,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                     bool mj; const double vj = height_of(j, mj);
                     rank += (vj < vi) || (vj == vi && j < i);
                 }
-                if (rank < sel) put_row(rank, i >> (2 * LOG), (i >> LOG) & MASK, i & MASK, P.binz, mi ? 1.0 : 0.0);
+                if (rank < sel) put_row(rank, G::rot_of(i), G::x_of(i), G::y_of(i), P.binz, mi ? 1.0 : 0.0);
             }
             zero_rows(total < sel ? total : sel);
         }
@@ -1465,12 +1465,11 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
         // candidate, so the height gathers of 32 candidates are in flight together.
         // candidate list + bucket-sorted index list: the (now idle) lane scratch, or the pair's slice of the global scratch
         // (a bin whose candidates fit the warp scratch keeps its lists there even when the global scratch exists; it is
-        // allocated whenever R * NPOSE > LIST_CAP_WS).  An entry is r << 2 LOG | b, b the bit of the pose in the rotation's set
-        // (b = ly * AY + lx: contour points are (column, row) = (ly, lx))
+        // allocated whenever R * NPOSE > LIST_CAP_WS).  An entry is r << 2 LOG | b, b the pose's bit (see Grid::list_pose)
         const bool spill = P.dlist && Ktot > CS::LIST_CAP_WS;
         const int LIST_CAP = spill ? R * G::NPOSE : CS::LIST_CAP_WS;         // >= Ktot
         uint16_t* list = spill ? P.dlist + (int64_t)env * 2 * (R * G::NPOSE) : reinterpret_cast<uint16_t*>(W_pts);
-        auto cell_of = [](int e) { const int b = e & (G::NPOSE - 1); return (e >> (2 * LOG)) * G::NPOSE + (b & MASK) * G::AY + (b >> LOG); };
+        auto put_entry = [&](int row, int e, double H, double V) { const auto p = G::list_pose(e); put_row(row, p.rot, p.x, p.y, H, V); };
         {
             for (int r = 0; r < R; ++r) {
                 const uint32_t* cb = cbits + r * G::BMW;
@@ -1487,9 +1486,8 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
             if (Ktot <= sel) {
                 for (int i = lane; i < Ktot; i += 32) {
                     const int e = list[i];
-                    const int b = e & (G::NPOSE - 1);
-                    bool m; const double H = height_of(cell_of(e), m);
-                    put_row(i, e >> (2 * LOG), b & MASK, b >> LOG, H, m ? 1.0 : 0.0);
+                    bool m; const double H = height_of(G::list_pose(e).cell, m);
+                    put_entry(i, e, H, m ? 1.0 : 0.0);
                 }
             } else {
                 // More candidates than rows: keep the `sel` lowest heights, ties by original order (stable
@@ -1504,7 +1502,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                 double hmin = POSZ_INVALID, hmax = -POSZ_INVALID;
                 int nvalid = 0;
                 for (int i = lane; i < Ktot; i += 32) {
-                    bool m; const double H = height_of(cell_of(list[i]), m);
+                    bool m; const double H = height_of(G::list_pose(list[i]).cell, m);
                     if (m) { hmin = fmin(hmin, H); hmax = fmax(hmax, H); ++nvalid; }
                 }
 #pragma unroll
@@ -1518,7 +1516,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                 for (int b = lane; b < RANK_BUCKETS; b += 32) hist[b] = 0;
                 __syncwarp();
                 for (int i = lane; i < Ktot; i += 32) {
-                    bool m; const double H = height_of(cell_of(list[i]), m);
+                    bool m; const double H = height_of(G::list_pose(list[i]).cell, m);
                     if (m) atomicAdd(&hist[bucket_of(H)], 1);
                 }
                 __syncwarp();
@@ -1539,7 +1537,7 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                 __syncwarp();
                 for (int i = lane; i < Ktot; i += 32) {
                     const int e = list[i];
-                    bool m; const double H = height_of(cell_of(e), m);
+                    bool m; const double H = height_of(G::list_pose(e).cell, m);
                     if (m) sorted[atomicAdd(&hist[RANK_BUCKETS + bucket_of(H)], 1)] = (uint16_t)e;
                 }
                 __syncwarp();
@@ -1547,9 +1545,8 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                 for (int i0 = 0; i0 < Ktot; i0 += 32) {
                     const int i = i0 + lane;
                     const int e = i < Ktot ? list[i] : 0;
-                    const int b = e & (G::NPOSE - 1);
                     bool m = false; double H = 0.0;
-                    if (i < Ktot) H = height_of(cell_of(e), m);
+                    if (i < Ktot) H = height_of(G::list_pose(e).cell, m);
                     const uint32_t inv = __ballot_sync(0xffffffffu, i < Ktot && !m);
                     if (i < Ktot && m) {
                         const int bk = bucket_of(H);
@@ -1558,14 +1555,14 @@ __global__ void __launch_bounds__(32 * EPC, (cand_min_ctas<EPC, G>())) irbpp_can
                             int rank = lo;
                             for (int t = lo; t < hi; ++t) {
                                 const int e2 = sorted[t];
-                                const double H2 = posz_g[cell_of(e2)];
+                                const double H2 = posz_g[G::list_pose(e2).cell];
                                 rank += (H2 < H) || (H2 == H && e2 < e);
                             }
-                            if (rank < sel) put_row(rank, e >> (2 * LOG), b & MASK, b >> LOG, H, 1.0);
+                            if (rank < sel) put_entry(rank, e, H, 1.0);
                         }
                     } else if (i < Ktot) {
                         const int rank = nvalid + inv_before + __popc(inv & ((1u << lane) - 1u));
-                        if (rank < sel) put_row(rank, e >> (2 * LOG), b & MASK, b >> LOG, H, 0.0);
+                        if (rank < sel) put_entry(rank, e, H, 0.0);
                     }
                     inv_before += __popc(inv);
                 }
