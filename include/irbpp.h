@@ -352,6 +352,44 @@ int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t ob
                   int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch, int64_t scratch_bytes,
                   void* stream);
 
+/* ---- the order network's forward pass and Agent.act (csrc/irbpp_order_actor.cuh) --------------------------------------
+ * DQNBPP.forward with args.level == 'order' and bufferSize k > 1 (model.py:355-383, 386-404: per buffer slot the shape
+ * feature and the map feature through gat_project_layer, one single-head graph-attention layer over the k slots of a
+ * bin, dueling heads over the slots) followed by Agent.act (agent.py:51-58), for N bins at once.  Handle-free, like
+ * irbpp_dqn_act, with the same weight conventions.  Supported: hidden_size 128, 2 <= k <= 32, 1 <= atoms <= 32, one
+ * attention head and layer with feed-forward width 128, the 32 x 32 heightmap. */
+typedef struct {
+    const float* conv1_w; const float* conv1_b;     /* heightEncoder.conv1 [16, 1, 4, 4], [16] */
+    const float* conv2_w; const float* conv2_b;     /* heightEncoder.conv2 [32, 16, 4, 4], [32] */
+    const float* conv3_w; const float* conv3_b;     /* heightEncoder.conv3 [4, 32, 3, 3], [4] */
+    const float* gat1_w; const float* gat1_b;       /* gat_project_layer.0 [256, 384], [256] */
+    const float* gat2_w; const float* gat2_b;       /* gat_project_layer.2 [128, 256], [128] */
+    const float* wq; const float* wk; const float* wv;  /* embedder.layers.0.0.module.W_query / W_key / W_val [128, 128] */
+    const float* wo_w; const float* wo_b;           /* embedder.layers.0.0.module.W_out [128, 128], [128] */
+    const float* ff1_w; const float* ff1_b;         /* embedder.layers.0.1.module.0 [128, 128], [128] */
+    const float* ff2_w; const float* ff2_b;         /* embedder.layers.0.1.module.2 [128, 128], [128] */
+    const float* fc_h_v_w; const float* fc_h_v_b;   /* fc_h_v [128, 128], [128] */
+    const float* fc_z_v_w; const float* fc_z_v_b;   /* fc_z_v [atoms, 128], [atoms] */
+    const float* fc_h_a_w; const float* fc_h_a_b;   /* fc_h_a [128, 128], [128] */
+    const float* fc_z_a_w; const float* fc_z_a_b;   /* fc_z_a [atoms, 128], [atoms] */
+    float negative_slope;                           /* of every LeakyReLU (nn.LeakyReLU default 0.01) */
+} irbpp_dqn_order_weights;
+
+/* Bytes of the scratch irbpp_dqn_order_act needs for N bins of k slots and S library shapes (-1 for bad sizes). */
+int64_t irbpp_dqn_order_scratch_bytes(int32_t N, int32_t k, int32_t S);
+
+/* obs float32 [N] rows of obs_stride >= k + 1024 (binPhy.py:229-230: k item ids as floats, the 32 x 32 heightmap);
+ * an id is read as (int) obs[b, j] and clamped to [0, S).  shape_features float32 [S, 128]: the shape feature
+ * (max over the sampled points of shapeEncoder, model.py:365-372) of every library shape.  support float32 [atoms].
+ * mask: float32 at mask[b * mask_row_stride + j * mask_elem_stride], or NULL for no masking (the reference passes
+ * None at this level).  Writes actions int64 [N] (argmax over the k slots of the masked expected value, first slot on
+ * ties, 0 for a fully masked bin) and, when sum_q_map is not NULL, the masked expected values float32 [N, k] (-inf
+ * where mask != 1).  scratch: irbpp_dqn_order_scratch_bytes bytes, 256-byte aligned. */
+int irbpp_dqn_order_act(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t k,
+                        const float* shape_features, int32_t S, const float* support, int32_t atoms, const float* mask,
+                        int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch,
+                        int64_t scratch_bytes, void* stream);
+
 /* Profiling aid: when enabled, thread 0 of every CTA adds the SM cycles it spent in each kernel phase
  * (0 scan kernel: load + apply action, 1 scan kernel: observation heightmap + scan + level bitmaps,
  * 2 candidates kernel: contour tasks, 3 candidates kernel: select / pad) to counters 0-3; counters 4-7 count

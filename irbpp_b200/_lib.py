@@ -53,6 +53,14 @@ class IrbppDqnWeights(ctypes.Structure):
                                          "fc_z_a_w", "fc_z_a_b")] + [("negative_slope", ctypes.c_float)]
 
 
+class IrbppDqnOrderWeights(ctypes.Structure):
+    """``irbpp_dqn_order_weights``: device pointers of the order network's effective weights, then the LeakyReLU slope."""
+    _fields_ = [(n, c_void_p) for n in ("conv1_w", "conv1_b", "conv2_w", "conv2_b", "conv3_w", "conv3_b", "gat1_w",
+                                         "gat1_b", "gat2_w", "gat2_b", "wq", "wk", "wv", "wo_w", "wo_b", "ff1_w", "ff1_b",
+                                         "ff2_w", "ff2_b", "fc_h_v_w", "fc_h_v_b", "fc_z_v_w", "fc_z_v_b", "fc_h_a_w",
+                                         "fc_h_a_b", "fc_z_a_w", "fc_z_a_b")] + [("negative_slope", ctypes.c_float)]
+
+
 # symbol -> (restype, argtypes); every symbol of include/irbpp.h appears here (checked by the tests)
 SIGNATURES = {
     "irbpp_abi_version": (c_i32, []),
@@ -91,6 +99,9 @@ SIGNATURES = {
     "irbpp_dqn_scratch_bytes": (c_i64, [c_i32, c_i32]),
     "irbpp_dqn_act": (c_i32, [ctypes.POINTER(IrbppDqnWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i32,
                               c_void_p, c_i64, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_dqn_order_scratch_bytes": (c_i64, [c_i32, c_i32, c_i32]),
+    "irbpp_dqn_order_act": (c_i32, [ctypes.POINTER(IrbppDqnOrderWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_i32,
+                                    c_void_p, c_i32, c_void_p, c_i64, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p]),
     "irbpp_replay_init": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p]),
     "irbpp_replay_append": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
                                     c_void_p, ctypes.c_float, c_void_p]),

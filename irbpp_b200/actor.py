@@ -12,6 +12,9 @@ A live module is read at every call (weights change after every ``learn`` and ``
 selects NoisyLinear's mode (train: ``mu + sigma * epsilon``, eval: ``mu``), built with the reference's own torch
 expression on the device.  A plain state dict (``Agent.save`` / ``torch.save(net.state_dict())``) is copied to the
 device once and takes the mode from ``train=``.
+
+``DeviceOrderActor`` does the same for the order network of the buffered configuration (``model.py:355-404``,
+``args.level == 'order'``, ``csrc/irbpp_order_actor.cuh``), the first call of the hierarchical loop.
 """
 import ctypes
 
@@ -51,41 +54,73 @@ _FIELDS = (("conv1_w", "heightEncoder.conv1.weight"), ("conv1_b", "heightEncoder
 SUPPORTED = "hidden_size 128, 1 <= atoms <= 32, selectedAction >= 1, a 32 x 32 heightmap (obs_len = sel * 5 + 9 + 1024)"
 
 
-def check_state_dict(sd):
-    """The number of atoms of a location-network state dict; ``ValueError`` for missing or misshapen keys."""
-    missing = [k for k in STATE_DICT_KEYS if k not in sd]
+def _check_keys(sd, keys, plain_shapes, level, supported):
+    """The number of atoms of a state dict; ``ValueError`` for missing or misshapen keys."""
+    missing = [k for k in keys if k not in sd]
     if missing:
-        raise ValueError("state dict lacks %s (a location-level DQNBPP has the keys %s)" % (missing, list(STATE_DICT_KEYS)))
+        raise ValueError("state dict lacks %s (a %s-level DQNBPP has the keys %s)" % (missing, level, list(keys)))
     zw = tuple(sd["fc_z_a.weight_mu"].shape)
     atoms = zw[0] if len(zw) == 2 else -1
     if not 1 <= atoms <= MAX_ATOMS:
-        raise ValueError("fc_z_a has %d atoms; supported: %s" % (atoms, SUPPORTED))
-    for k, shape in PLAIN_SHAPES.items():
+        raise ValueError("fc_z_a has %d atoms; supported: %s" % (atoms, supported))
+    for k, shape in plain_shapes.items():
         if tuple(sd[k].shape) != shape:
-            raise ValueError("%s has shape %s, expected %s; supported: %s" % (k, tuple(sd[k].shape), shape, SUPPORTED))
+            raise ValueError("%s has shape %s, expected %s; supported: %s" % (k, tuple(sd[k].shape), shape, supported))
     for m, (n_in, n_out) in NOISY_IN_OUT.items():
         n_out = atoms if n_out is None else n_out
         for s in NOISY_SUFFIXES:
             want = (n_out, n_in) if s.startswith("weight") else (n_out,)
             if tuple(sd["%s.%s" % (m, s)].shape) != want:
                 raise ValueError("%s.%s has shape %s, expected %s; supported: %s" % (m, s, tuple(sd["%s.%s" % (m, s)].shape),
-                                                                                   want, SUPPORTED))
+                                                                                   want, supported))
     return atoms
 
 
-class DeviceActor(object):
-    """``Agent.act`` for every bin through ``irbpp_dqn_act``.
+def check_state_dict(sd):
+    """The number of atoms of a location-network state dict; ``ValueError`` for missing or misshapen keys."""
+    return _check_keys(sd, STATE_DICT_KEYS, PLAIN_SHAPES, "location", SUPPORTED)
 
-    ``net_or_state_dict``: a location-level ``DQNBPP`` (or any module with its ``state_dict`` keys, read live at every
-    call) or a state dict (copied to the device once; ``train`` picks NoisyLinear's mode, default True as
-    ``trainer.py`` acts).  ``clouds``: the ``DeviceShapeClouds`` that serves the next item's point-cloud feature (may be
-    None when every call passes ``shape_feature=``).  ``support``: the atoms' values (``Agent.support``)."""
 
-    def __init__(self, net_or_state_dict, clouds, support, train=None, device=None):
+# ---- the order level (model.py:355-383 with args.level == 'order', csrc/irbpp_order_actor.cuh) ----
+MAX_BUFFER = 32
+_ATT = "embedder.layers.0.0.module."
+_FFN = "embedder.layers.0.1.module."
+# key -> shape of the keys the order kernels read (init_candidate_embed and project_layer are in the reference's dict
+# but unused at this level)
+ORDER_PLAIN_SHAPES = dict(
+    [(k, s) for k, s in PLAIN_SHAPES.items() if k.startswith(("heightEncoder.", "shapeEncoder."))] +
+    [("gat_project_layer.0.weight", (256, 384)), ("gat_project_layer.0.bias", (256,)),
+     ("gat_project_layer.2.weight", (EMB, 256)), ("gat_project_layer.2.bias", (EMB,)),
+     (_ATT + "W_query.weight", (EMB, EMB)), (_ATT + "W_key.weight", (EMB, EMB)), (_ATT + "W_val.weight", (EMB, EMB)),
+     (_ATT + "W_out.weight", (EMB, EMB)), (_ATT + "W_out.bias", (EMB,)),
+     (_FFN + "0.weight", (EMB, EMB)), (_FFN + "0.bias", (EMB,)), (_FFN + "2.weight", (EMB, EMB)), (_FFN + "2.bias", (EMB,))])
+ORDER_STATE_DICT_KEYS = tuple(ORDER_PLAIN_SHAPES) + tuple("%s.%s" % (m, s) for m in NOISY for s in NOISY_SUFFIXES)
+# irbpp_dqn_order_weights field -> state_dict key
+_ORDER_FIELDS = (_FIELDS[:6] + (
+    ("gat1_w", "gat_project_layer.0.weight"), ("gat1_b", "gat_project_layer.0.bias"),
+    ("gat2_w", "gat_project_layer.2.weight"), ("gat2_b", "gat_project_layer.2.bias"),
+    ("wq", _ATT + "W_query.weight"), ("wk", _ATT + "W_key.weight"), ("wv", _ATT + "W_val.weight"),
+    ("wo_w", _ATT + "W_out.weight"), ("wo_b", _ATT + "W_out.bias"), ("ff1_w", _FFN + "0.weight"), ("ff1_b", _FFN + "0.bias"),
+    ("ff2_w", _FFN + "2.weight"), ("ff2_b", _FFN + "2.bias")) + _FIELDS[14:])
+ORDER_SUPPORTED = ("hidden_size 128, one attention head and layer with feed-forward width 128, 2 <= bufferSize <= 32, "
+                   "1 <= atoms <= 32, a 32 x 32 heightmap (obs_len = bufferSize + 1024)")
+
+
+def check_order_state_dict(sd):
+    """The number of atoms of an order-network state dict; ``ValueError`` for missing or misshapen keys."""
+    return _check_keys(sd, ORDER_STATE_DICT_KEYS, ORDER_PLAIN_SHAPES, "order", ORDER_SUPPORTED)
+
+
+class _NetworkSource(object):
+    """The weights a device actor reads: a module (read live at every call, its ``training`` flag picks NoisyLinear's
+    mode) or a state dict (copied to the device once, ``train`` picks the mode, default True).  ``keys``: the state
+    dict keys the kernels read; ``check(sd)`` validates them and returns the number of atoms."""
+
+    def __init__(self, net_or_state_dict, support, train, device, keys, check):
         import torch
         self._torch = torch
         self._lib = _lib.load()
-        self.clouds = clouds
+        self._keys = keys
         if isinstance(net_or_state_dict, torch.nn.Module):
             self.net = net_or_state_dict
             if train is not None:
@@ -96,10 +131,10 @@ class DeviceActor(object):
             sd = net_or_state_dict
             if not hasattr(sd, "keys"):
                 raise ValueError("expected a DQNBPP module or its state dict, got %s" % type(sd).__name__)
-            for k in STATE_DICT_KEYS:
+            for k in keys:
                 if k in sd and not isinstance(sd[k], torch.Tensor):
                     raise ValueError("state dict entry %s is not a tensor" % k)
-        self.atoms = check_state_dict(sd)
+        self.atoms = check(sd)
         if not isinstance(support, torch.Tensor) or not support.is_cuda:
             raise ValueError("support must be a CUDA tensor of the %d atoms' values" % self.atoms)
         self.device = torch.device(device) if device is not None else support.device
@@ -110,27 +145,25 @@ class DeviceActor(object):
         self.support = support.detach().to(torch.float32).reshape(-1).contiguous()
         if self.net is None:
             self.train = True if train is None else bool(train)
-            self._static = {k: sd[k].detach().to(self.device, torch.float32).contiguous() for k in STATE_DICT_KEYS}
+            self._static = {k: sd[k].detach().to(self.device, torch.float32).contiguous() for k in keys}
         self._scratch = None
         self._keep = None
 
-    # ---- weights ----
     def _state(self):
         if self.net is None:
             return self._static, self.train
         sd = self.net.state_dict()
-        for k in STATE_DICT_KEYS:
+        for k in self._keys:
             if sd[k].device != self.device:
                 raise ValueError("network weights live on %s, the actor on %s" % (sd[k].device, self.device))
         return sd, self.net.training
 
-    def effective_weights(self):
-        """The weights the kernels use, by field of ``irbpp_dqn_weights``: NoisyLinear layers with the torch expression
-        of model.py:224-228 for the current mode (rebuilt at every call)."""
-        torch = self._torch
+    def _effective(self, plain):
+        """The state dict's ``plain`` keys and, for every NoisyLinear layer m, ``m.weight`` / ``m.bias`` built with the
+        torch expression of model.py:224-228 for the current mode (at every call)."""
         sd, train = self._state()
         out = {}
-        with torch.no_grad():
+        with self._torch.no_grad():
             for m in NOISY:
                 if train:
                     w = sd[m + ".weight_mu"] + sd[m + ".weight_sigma"] * sd[m + ".weight_epsilon"]
@@ -138,8 +171,35 @@ class DeviceActor(object):
                 else:
                     w, b = sd[m + ".weight_mu"], sd[m + ".bias_mu"]
                 out[m + ".weight"], out[m + ".bias"] = w, b
-            for k in PLAIN_SHAPES:
+            for k in plain:
                 out[k] = sd[k]
+        return out
+
+    def _scratch_of(self, need):
+        if self._scratch is None or self._scratch.numel() < need:
+            self._scratch = self._torch.empty(need, dtype=self._torch.uint8, device=self.device)
+        return self._scratch
+
+
+class DeviceActor(_NetworkSource):
+    """``Agent.act`` for every bin through ``irbpp_dqn_act``.
+
+    ``net_or_state_dict``: a location-level ``DQNBPP`` (or any module with its ``state_dict`` keys, read live at every
+    call) or a state dict (copied to the device once; ``train`` picks NoisyLinear's mode, default True as
+    ``trainer.py`` acts).  ``clouds``: the ``DeviceShapeClouds`` that serves the next item's point-cloud feature (may be
+    None when every call passes ``shape_feature=``).  ``support``: the atoms' values (``Agent.support``)."""
+
+    def __init__(self, net_or_state_dict, clouds, support, train=None, device=None):
+        _NetworkSource.__init__(self, net_or_state_dict, support, train, device, STATE_DICT_KEYS, check_state_dict)
+        self.clouds = clouds
+
+    # ---- weights ----
+    def effective_weights(self):
+        """The weights the kernels use, by field of ``irbpp_dqn_weights``: NoisyLinear layers with the torch expression
+        of model.py:224-228 for the current mode (rebuilt at every call)."""
+        torch = self._torch
+        with torch.no_grad():
+            out = self._effective(PLAIN_SHAPES)
             ws = {f: out[k].detach().to(torch.float32).contiguous() for f, k in _FIELDS}
             enc = tuple(out[k].detach().to(torch.float32).contiguous() for k in (
                 "shapeEncoder.linear1.weight", "shapeEncoder.linear1.bias", "shapeEncoder.linear2.weight",
@@ -183,9 +243,7 @@ class DeviceActor(object):
             if mask.dtype != torch.float32:
                 mask = mask.to(torch.float32)
             m_ptr, m_row, m_elem = mask.data_ptr(), mask.stride(0), mask.stride(1)
-        need = int(self._lib.irbpp_dqn_scratch_bytes(N, sel))
-        if self._scratch is None or self._scratch.numel() < need:
-            self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+        self._scratch_of(int(self._lib.irbpp_dqn_scratch_bytes(N, sel)))
         actions = torch.empty(N, dtype=torch.int64, device=self.device)
         q = torch.empty((N, sel), dtype=torch.float32, device=self.device) if want_q else None
         w = _lib.IrbppDqnWeights(*([ws[f].data_ptr() for f, _ in _FIELDS] + [ctypes.c_float(0.01)]))
@@ -205,3 +263,89 @@ class DeviceActor(object):
     def q_values(self, state, mask=None, shape_feature=None):
         """The masked ``sum_q_map`` of agent.py:53-57: float32 ``[N, sel]`` (-inf where ``mask != 1``)."""
         return self._run(state, mask, shape_feature, True)[1]
+
+
+class DeviceOrderActor(_NetworkSource):
+    """``Agent.act`` of the order network (``DQNBPP`` with ``args.level == 'order'``, ``bufferSize`` k > 1) for every
+    bin through ``irbpp_dqn_order_act``: the first call of the hierarchical loop (``trainer.py:261-281``,
+    ``tools.py:361-387``)::
+
+        order_actor = DeviceOrderActor(orderDQN.online_net, clouds, orderDQN.support)
+        orderAction = order_actor.act(orderState)        # drop-in for orderDQN.act(orderState, None)
+
+    ``net_or_state_dict``, ``train`` and ``support`` as for ``DeviceActor``.  ``clouds``: the ``DeviceShapeClouds`` (or
+    ``pointnet.OrderShapeClouds``, the order level's own point rule) whose ``features`` on the ids ``arange(S)`` give the
+    per-shape table the kernels gather from, one index set per act; may be None when every call passes
+    ``shape_features=`` (float32 ``[S, 128]`` on the actor's device)."""
+
+    def __init__(self, net_or_state_dict, clouds, support, train=None, device=None):
+        _NetworkSource.__init__(self, net_or_state_dict, support, train, device, ORDER_STATE_DICT_KEYS,
+                                check_order_state_dict)
+        self.clouds = clouds
+
+    def effective_weights(self):
+        """The weights the kernels use, by field of ``irbpp_dqn_order_weights``, and the shape encoder's tensors."""
+        torch = self._torch
+        with torch.no_grad():
+            out = self._effective(ORDER_PLAIN_SHAPES)
+            ws = {f: out[k].detach().to(torch.float32).contiguous() for f, k in _ORDER_FIELDS}
+            enc = tuple(out[k].detach().to(torch.float32).contiguous() for k in (
+                "shapeEncoder.linear1.weight", "shapeEncoder.linear1.bias", "shapeEncoder.linear2.weight",
+                "shapeEncoder.linear2.bias"))
+        return ws, enc
+
+    def _check_state(self, state):
+        torch = self._torch
+        if not isinstance(state, torch.Tensor) or not state.is_cuda:
+            raise ValueError("order state must be a CUDA tensor [N, bufferSize + 1024]")
+        if state.device != self.device:
+            raise ValueError("order state lives on %s, the actor on %s" % (state.device, self.device))
+        if state.dim() != 2 or state.dtype != torch.float32:
+            raise ValueError("order state must be float32 [N, bufferSize + 1024], got %s %s" % (state.dtype, tuple(state.shape)))
+        k = state.shape[1] - HM * HM
+        if not 2 <= k <= MAX_BUFFER:
+            raise ValueError("order observation width %d is not bufferSize + 1024; supported: %s" % (state.shape[1], ORDER_SUPPORTED))
+        return state if state.stride(1) == 1 else state.contiguous(), k
+
+    def _run(self, state, mask, shape_features, want_q):
+        torch = self._torch
+        state, k = self._check_state(state)
+        N = state.shape[0]
+        ws, enc = self.effective_weights()
+        if shape_features is None:
+            if self.clouds is None:
+                raise ValueError("no DeviceShapeClouds given: pass shape_features=")
+            ids = torch.arange(self.clouds.S, dtype=torch.int32, device=self.device)
+            shape_features = self.clouds.features(ids, enc + (0.01,))
+        if (not isinstance(shape_features, torch.Tensor) or shape_features.device != self.device
+                or shape_features.dim() != 2 or shape_features.shape[1] != EMB or shape_features.shape[0] < 1):
+            raise ValueError("shape_features must be a tensor [S, %d] on %s" % (EMB, self.device))
+        shape_features = shape_features.detach().to(torch.float32).contiguous()
+        S = shape_features.shape[0]
+        m_ptr, m_row, m_elem = 0, 0, 0
+        if mask is not None:
+            if not isinstance(mask, torch.Tensor) or mask.device != self.device or tuple(mask.shape) != (N, k):
+                raise ValueError("mask must be a tensor [%d, %d] on %s" % (N, k, self.device))
+            if mask.dtype != torch.float32:
+                mask = mask.to(torch.float32)
+            m_ptr, m_row, m_elem = mask.data_ptr(), mask.stride(0), mask.stride(1)
+        scratch = self._scratch_of(int(self._lib.irbpp_dqn_order_scratch_bytes(N, k, S)))
+        actions = torch.empty(N, dtype=torch.int64, device=self.device)
+        q = torch.empty((N, k), dtype=torch.float32, device=self.device) if want_q else None
+        w = _lib.IrbppDqnOrderWeights(*([ws[f].data_ptr() for f, _ in _ORDER_FIELDS] + [ctypes.c_float(0.01)]))
+        rc = self._lib.irbpp_dqn_order_act(ctypes.byref(w), state.data_ptr(), state.stride(0), N, k, shape_features.data_ptr(),
+                                           S, self.support.data_ptr(), self.atoms, m_ptr, m_row, m_elem, actions.data_ptr(),
+                                           q.data_ptr() if q is not None else 0, scratch.data_ptr(), scratch.numel(),
+                                           torch.cuda.current_stream(self.device).cuda_stream)
+        _lib.check(self._lib, None, rc)
+        self._keep = (ws, enc, shape_features, mask, state)    # alive until the next call: the launches are asynchronous
+        return actions, q
+
+    def act(self, order_state, mask=None, shape_features=None):
+        """``orderDQN.act(orderState, mask)``: int64 ``[N]`` slots on the device.  ``mask=None`` masks nothing, as the
+        reference acts at this level."""
+        return self._run(order_state, mask, shape_features, False)[0]
+
+    def q_values(self, order_state, mask=None, shape_features=None):
+        """The masked ``sum_q_map`` of agent.py:53-57: float32 ``[N, k]`` (-inf where ``mask != 1``)."""
+        return self._run(order_state, mask, shape_features, True)[1]

@@ -23,6 +23,7 @@
 #include "irbpp_pack.cuh"
 #include "irbpp_replay.cuh"
 #include "irbpp_actor.cuh"
+#include "irbpp_order_actor.cuh"
 
 using namespace irbpp;
 
@@ -1101,6 +1102,53 @@ int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t ob
     cudaStream_t s = (cudaStream_t)stream;
     irbpp_actor_bin_kernel<<<N, AC_THREADS, 0, s>>>(A);
     irbpp_actor_rows_kernel<<<N, AC_THREADS, AC_ROWS_SMEM_BYTES, s>>>(A);
+    return launch_status();
+}
+
+// ---- the order network's forward pass and Agent.act (csrc/irbpp_order_actor.cuh) ---------------------------------
+int64_t irbpp_dqn_order_scratch_bytes(int32_t N, int32_t k, int32_t S) {
+    if (N <= 0 || k < 2 || k > OA_MAXK || S <= 0) return -1;
+    return order_scratch_bytes(N, S);
+}
+
+int irbpp_dqn_order_act(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t k,
+                        const float* shape_features, int32_t S, const float* support, int32_t atoms, const float* mask,
+                        int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch,
+                        int64_t scratch_bytes, void* stream) {
+    if (!weights || !obs || !shape_features || !support || !actions || !scratch) return fail(nullptr, IRBPP_EINVAL, "null order act argument");
+    if (N <= 0 || S <= 0) return fail(nullptr, IRBPP_EINVAL, "need N >= 1 bins and S >= 1 shapes (N %d, S %d)", N, S);
+    if (k < 2 || k > OA_MAXK) return fail(nullptr, IRBPP_EINVAL, "buffer size k %d outside [2, %d]", k, OA_MAXK);
+    if (atoms < 1 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [1, %d]", atoms, AC_MAXATOMS);
+    if (obs_stride < (int64_t)k + AC_HM * AC_HM)
+        return fail(nullptr, IRBPP_EINVAL, "observation stride %lld < k + 1024", (long long)obs_stride);
+    if (scratch_bytes < order_scratch_bytes(N, S))
+        return fail(nullptr, IRBPP_EINVAL, "scratch of %lld bytes < %lld", (long long)scratch_bytes, (long long)order_scratch_bytes(N, S));
+    if (reinterpret_cast<uintptr_t>(scratch) & 255) return fail(nullptr, IRBPP_EINVAL, "scratch not 256-byte aligned");
+    const irbpp_dqn_order_weights& w = *weights;
+    const float* ptrs[] = {w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.gat1_w, w.gat1_b, w.gat2_w,
+                           w.gat2_b, w.wq, w.wk, w.wv, w.wo_w, w.wo_b, w.ff1_w, w.ff1_b, w.ff2_w, w.ff2_b, w.fc_h_v_w,
+                           w.fc_h_v_b, w.fc_z_v_w, w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b};
+    for (const float* p : ptrs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null weight pointer");
+    OrderParams A;
+    memset(&A, 0, sizeof(A));
+    A.w = OrderWeights{w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.gat1_w, w.gat1_b, w.gat2_w,
+                       w.gat2_b, w.wq, w.wk, w.wv, w.wo_w, w.wo_b, w.ff1_w, w.ff1_b, w.ff2_w, w.ff2_b, w.fc_h_v_w,
+                       w.fc_h_v_b, w.fc_z_v_w, w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b, w.negative_slope};
+    A.obs = obs; A.obs_stride = obs_stride; A.N = N; A.k = k; A.S = S; A.atoms = atoms;
+    A.shape_features = shape_features; A.support = support;
+    A.mask = mask; A.mask_row = mask_row_stride; A.mask_elem = mask_elem_stride;
+    A.actions = actions; A.sum_q = sum_q_map;
+    order_scratch_layout(A, scratch);
+    const int dev = device_of(obs);
+    DeviceGuard guard(dev);
+    cudaError_t e = raise_dynamic_smem(dev, (const void*)irbpp_order_slots_kernel, OA_SLOTS_SMEM_BYTES);
+    if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "slots kernel set-up: %s", cudaGetErrorString(e));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int per = AC_TM / k;
+    irbpp_order_table_kernel<<<S, AC_THREADS, 0, s>>>(A);
+    irbpp_order_bin_kernel<<<N, AC_THREADS, 0, s>>>(A);
+    irbpp_order_slots_kernel<<<(N + per - 1) / per, AC_THREADS, OA_SLOTS_SMEM_BYTES, s>>>(A);
     return launch_status();
 }
 

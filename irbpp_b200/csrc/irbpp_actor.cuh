@@ -197,26 +197,21 @@ __device__ __forceinline__ void ac_layer(const float* in, int ld_in, const float
             }
 }
 
-// ---- per-bin kernel ------------------------------------------------------------------------------------------------
-// One CTA per bin: heightEncoder (model.py:258-264, LeakyReLU after every conv), the flatten in C, H, W order, u_b and
-// the list of rows with mask == 1 (model.py:321-322, 347-349: every other row's embedding is zeroed).
-__global__ void __launch_bounds__(AC_THREADS) irbpp_actor_bin_kernel(const ActorParams A) {
-    __shared__ __align__(16) float hm[AC_HM * AC_HM];          // [1][32][32]
-    __shared__ __align__(16) float c1[16 * 16 * 16];            // [16][16][16]
-    __shared__ __align__(16) float c2[32 * 8 * 8];              // [32][8][8]
-    __shared__ __align__(16) float x[384];                      // shape_feature | map_feature
-    const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const float slope = A.w.slope;
-    const float* ob = A.obs + (int64_t)b * A.obs_stride;
-    const float* hsrc = ob + (int64_t)A.sel * 5 + 9;            // model.py:181
-    for (int i = tid; i < AC_HM * AC_HM; i += AC_THREADS) hm[i] = hsrc[i];
-    if (tid < AC_EMB) x[tid] = A.shape_feature[(int64_t)b * AC_EMB + tid];
+// ---- heightEncoder ---------------------------------------------------------------------------------------------------
+// heightEncoder (model.py:258-264, LeakyReLU after every conv) of the 32 x 32 heightmap the CTA's threads have stored
+// in hm (the barrier is here), by the AC_THREADS threads of a CTA; the 256 map features, flattened in C, H, W order,
+// go to map[0:256].  hm, c1 and c2 are the CTA's shared buffers.  Shared by the location and order levels (W:
+// ActorWeights or OrderWeights, same conv fields).
+template <class W>
+__device__ __forceinline__ void ac_height_encoder(const W& w, float* hm, float* c1, float* c2, float* map) {
+    const int tid = threadIdx.x;
+    const float slope = w.slope;
     __syncthreads();
     // conv1: 1 -> 16, k4, stride 2, pad 1: 32 -> 16
     for (int o = tid; o < 16 * 16 * 16; o += AC_THREADS) {
         const int co = o >> 8, y = (o >> 4) & 15, xx = o & 15;
-        float acc = A.w.conv1_b[co];
-        const float* wk = A.w.conv1_w + co * 16;
+        float acc = w.conv1_b[co];
+        const float* wk = w.conv1_w + co * 16;
         for (int ky = 0; ky < 4; ++ky) {
             const int iy = 2 * y - 1 + ky;
             if (iy < 0 || iy >= AC_HM) continue;
@@ -232,9 +227,9 @@ __global__ void __launch_bounds__(AC_THREADS) irbpp_actor_bin_kernel(const Actor
     // conv2: 16 -> 32, k4, stride 2, pad 1: 16 -> 8
     for (int o = tid; o < 32 * 8 * 8; o += AC_THREADS) {
         const int co = o >> 6, y = (o >> 3) & 7, xx = o & 7;
-        float acc = A.w.conv2_b[co];
+        float acc = w.conv2_b[co];
         for (int ci = 0; ci < 16; ++ci) {
-            const float* wk = A.w.conv2_w + (co * 16 + ci) * 16;
+            const float* wk = w.conv2_w + (co * 16 + ci) * 16;
             const float* in = c1 + ci * 256;
             for (int ky = 0; ky < 4; ++ky) {
                 const int iy = 2 * y - 1 + ky;
@@ -249,12 +244,12 @@ __global__ void __launch_bounds__(AC_THREADS) irbpp_actor_bin_kernel(const Actor
         c2[o] = ac_leaky(acc, slope);
     }
     __syncthreads();
-    // conv3: 32 -> 4, k3, stride 1, pad 1: 8 -> 8; flattened (C, H, W) after the shape feature
+    // conv3: 32 -> 4, k3, stride 1, pad 1: 8 -> 8; flattened (C, H, W)
     {
         const int o = tid, co = o >> 6, y = (o >> 3) & 7, xx = o & 7;
-        float acc = A.w.conv3_b[co];
+        float acc = w.conv3_b[co];
         for (int ci = 0; ci < 32; ++ci) {
-            const float* wk = A.w.conv3_w + (co * 32 + ci) * 9;
+            const float* wk = w.conv3_w + (co * 32 + ci) * 9;
             const float* in = c2 + ci * 64;
             for (int ky = 0; ky < 3; ++ky) {
                 const int iy = y - 1 + ky;
@@ -266,9 +261,25 @@ __global__ void __launch_bounds__(AC_THREADS) irbpp_actor_bin_kernel(const Actor
                 }
             }
         }
-        x[AC_EMB + o] = ac_leaky(acc, slope);
+        map[o] = ac_leaky(acc, slope);
     }
     __syncthreads();
+}
+
+// ---- per-bin kernel ------------------------------------------------------------------------------------------------
+// One CTA per bin: heightEncoder, u_b and the list of rows with mask == 1 (model.py:321-322, 347-349: every other
+// row's embedding is zeroed).
+__global__ void __launch_bounds__(AC_THREADS) irbpp_actor_bin_kernel(const ActorParams A) {
+    __shared__ __align__(16) float hm[AC_HM * AC_HM];          // [1][32][32]
+    __shared__ __align__(16) float c1[16 * 16 * 16];            // [16][16][16]
+    __shared__ __align__(16) float c2[32 * 8 * 8];              // [32][8][8]
+    __shared__ __align__(16) float x[384];                      // shape_feature | map_feature
+    const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const float* ob = A.obs + (int64_t)b * A.obs_stride;
+    const float* hsrc = ob + (int64_t)A.sel * 5 + 9;            // model.py:181
+    for (int i = tid; i < AC_HM * AC_HM; i += AC_THREADS) hm[i] = hsrc[i];
+    if (tid < AC_EMB) x[tid] = A.shape_feature[(int64_t)b * AC_EMB + tid];
+    ac_height_encoder(A.w, hm, c1, c2, x + AC_EMB);
     // u_b = proj1_w[:, 0:384] . x + proj1_b: one warp per output, lanes over k (coalesced rows of the weight)
     for (int j = warp; j < AC_PROJ; j += AC_THREADS / 32) {
         const float* wr = A.w.proj1_w + (int64_t)j * 512;

@@ -118,3 +118,49 @@ class DeviceShapeClouds(object):
         if counter is None:
             self.counter += 1
         return out
+
+
+# ---- the order level's point rule (model.py:240-244, 301-306, 365-368, 401-403) ----
+ORDER_ARRAY_POINTS = 10000          # arrayPointNum: the points of each shape's subsample
+ORDER_REDRAW = 1000                 # the subsample is redrawn every 1000 forward passes
+_SUBSAMPLE_STREAM = 1 << 40         # generator counters of the subsamples, apart from those of the acts (< 2**40)
+
+
+def order_point_indices(seed, act, n_points, num_cloud_points):
+    """Host mirror of ``OrderShapeClouds``: the cloud points (indices into ``shapeArray``'s second axis) of act
+    ``act``, the act's draw mapped through the subsample of its epoch ``act // 1000``."""
+    sub = pn_indices(seed, _SUBSAMPLE_STREAM + act // ORDER_REDRAW, ORDER_ARRAY_POINTS,
+                     min(num_cloud_points, ORDER_ARRAY_POINTS))
+    return sub[pn_indices(seed, act, n_points, ORDER_ARRAY_POINTS)]
+
+
+class OrderShapeClouds(object):
+    """The order network's point rule over a ``DeviceShapeClouds`` (opt-in; the default path samples the whole cloud).
+
+    The reference's order level keeps a subsample of 10 000 points per shape, drawn with replacement from the first
+    10 000 points of each cloud (``np.random.randint(self.shapeArray.shape[1])`` there reads the subsample's own
+    size) and redrawn every 1000 forward passes; each forward draws ``samplePointsNum`` of those 10 000.  Here both
+    draws come from the counter-based generator of ``DeviceShapeClouds`` (``order_point_indices`` mirrors them on the
+    host).  A cloud of fewer than 10 000 points is subsampled over all its points (the reference raises there)."""
+
+    def __init__(self, clouds):
+        self.clouds = clouds
+        self.S, self.device, self.item_col = clouds.S, clouds.device, clouds.item_col
+        self.counter = 0                    # acts served so far
+        self._epoch, self._sub = None, None
+
+    def features(self, obs_or_ids, encoder, counter=None):
+        """``DeviceShapeClouds.features`` on the current subsample: float32 ``[B, 128]``."""
+        torch = self.clouds._torch
+        c = self.counter if counter is None else int(counter)
+        epoch = c // ORDER_REDRAW
+        if epoch != self._epoch:
+            src = self.clouds
+            idx = pn_indices(src.seed, _SUBSAMPLE_STREAM + epoch, ORDER_ARRAY_POINTS, min(src.P, ORDER_ARRAY_POINTS))
+            self._sub = DeviceShapeClouds(src.shape_array[:, torch.as_tensor(idx, device=src.device)], device=src.device,
+                                          n_points=src.n_points, seed=src.seed, item_col=src.item_col)
+            self._epoch = epoch
+        out = self._sub.features(obs_or_ids, encoder, counter=c)
+        if counter is None:
+            self.counter += 1
+        return out
