@@ -390,6 +390,34 @@ int irbpp_dqn_order_act(const irbpp_dqn_order_weights* weights, const float* obs
                         int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch,
                         int64_t scratch_bytes, void* stream);
 
+/* ---- the target distribution of Agent.learn (csrc/irbpp_learn.cuh) ---------------------------------------------------
+ * The no-grad target half of Agent.learn (agent.py:94-115) for B sampled transitions, run over the TARGET net's
+ * effective weights (after target_net.reset_noise()): the forward pass of irbpp_dqn_act / irbpp_dqn_order_act on the
+ * next states, then for every transition b, with a* = next_actions[b] (the unmasked online argmax of agent.py:90-92,
+ * e.g. irbpp_dqn_act with mask = NULL), p = p(s', a*; target) and the projection of agent.py:100-115:
+ *   Tz = clamp(returns[b] + nonterminals[b] * discount_n * z, v_min, v_max), b_z = (Tz - v_min) / dz,
+ *   dz = (v_max - v_min) / (atoms - 1) formed in double (agent.py:20), l = floor(b_z), u = ceil(b_z) with the two
+ *   fix-ups of agent.py:108-109, m[l] += p (u - b_z), m[u] += p (b_z - l).
+ * Arithmetic follows torch's float32 CUDA evaluation (discount_n, v_min, v_max enter as float32; the division is a
+ * multiplication by the float32 reciprocal of dz, as torch's CUDA kernel does it; b_z is capped at atoms - 1, which
+ * float32 can pass by an ulp at Tz = v_max, where torch adds into the next row); the additions into m run in a fixed
+ * order (every l-contribution in atom order, then every u-contribution), so m is deterministic.  Writes m float32
+ * [B, atoms] and, when p_next is not NULL, p float32 [B, atoms].  A value of next_actions outside the rows (slots) is
+ * clamped to [0, selected_action) ([0, k)), as item ids are.  returns, nonterminals: float32 [B] (the [B, 1]
+ * nonterminals of PrioritizedReplayBank.sample are contiguous).  Supported: 2 <= atoms <= 32 (the reference divides
+ * by zero at one atom), v_max > v_min, B >= 1, and the size rules of the act entry point.  scratch: the act scratch
+ * (irbpp_dqn_scratch_bytes(B, selected_action) / irbpp_dqn_order_scratch_bytes(B, k, S)). */
+int irbpp_dqn_target(const irbpp_dqn_weights* target, const float* next_obs, int64_t obs_stride, int32_t B,
+                     int32_t selected_action, const float* shape_feature, const float* support, int32_t atoms,
+                     const int64_t* next_actions, const float* returns, const float* nonterminals, double discount_n,
+                     double v_min, double v_max, float* m, float* p_next, void* scratch, int64_t scratch_bytes,
+                     void* stream);
+int irbpp_dqn_order_target(const irbpp_dqn_order_weights* target, const float* next_obs, int64_t obs_stride, int32_t B,
+                           int32_t k, const float* shape_features, int32_t S, const float* support, int32_t atoms,
+                           const int64_t* next_actions, const float* returns, const float* nonterminals,
+                           double discount_n, double v_min, double v_max, float* m, float* p_next, void* scratch,
+                           int64_t scratch_bytes, void* stream);
+
 /* Profiling aid: when enabled, thread 0 of every CTA adds the SM cycles it spent in each kernel phase
  * (0 scan kernel: load + apply action, 1 scan kernel: observation heightmap + scan + level bitmaps,
  * 2 candidates kernel: contour tasks, 3 candidates kernel: select / pad) to counters 0-3; counters 4-7 count

@@ -102,6 +102,12 @@ SIGNATURES = {
     "irbpp_dqn_order_scratch_bytes": (c_i64, [c_i32, c_i32, c_i32]),
     "irbpp_dqn_order_act": (c_i32, [ctypes.POINTER(IrbppDqnOrderWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_i32,
                                     c_void_p, c_i32, c_void_p, c_i64, c_i64, c_void_p, c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_dqn_target": (c_i32, [ctypes.POINTER(IrbppDqnWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p, c_i32,
+                                 c_void_p, c_void_p, c_void_p, c_f64, c_f64, c_f64, c_void_p, c_void_p, c_void_p, c_i64,
+                                 c_void_p]),
+    "irbpp_dqn_order_target": (c_i32, [ctypes.POINTER(IrbppDqnOrderWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_i32,
+                                       c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_f64, c_f64, c_f64, c_void_p,
+                                       c_void_p, c_void_p, c_i64, c_void_p]),
     "irbpp_replay_init": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p]),
     "irbpp_replay_append": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
                                     c_void_p, ctypes.c_float, c_void_p]),

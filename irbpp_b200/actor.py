@@ -175,6 +175,24 @@ class _NetworkSource(object):
                 out[k] = sd[k]
         return out
 
+    def _target_inputs(self, N, next_actions, returns, nonterminals, v_min, v_max, with_p):
+        """The target pass's per-transition inputs as contiguous device vectors, and its outputs ``m`` and ``p_next``
+        (None unless ``with_p``)."""
+        torch = self._torch
+        if self.atoms < 2:
+            raise ValueError("the target distribution needs 2 <= atoms <= %d (the network has %d)" % (MAX_ATOMS, self.atoms))
+        if not float(v_max) > float(v_min):
+            raise ValueError("need v_max > v_min, got v_min %r, v_max %r" % (v_min, v_max))
+        out = []
+        for name, x, dtype in (("next_actions", next_actions, torch.int64), ("returns", returns, torch.float32),
+                               ("nonterminals", nonterminals, torch.float32)):
+            if not isinstance(x, torch.Tensor) or x.device != self.device or x.numel() != N:
+                raise ValueError("%s must be a tensor of %d values on %s" % (name, N, self.device))
+            out.append(x.detach().reshape(N).to(dtype).contiguous())
+        m = torch.empty((N, self.atoms), dtype=torch.float32, device=self.device)
+        p = torch.empty((N, self.atoms), dtype=torch.float32, device=self.device) if with_p else None
+        return out + [m, p]
+
     def _scratch_of(self, need):
         if self._scratch is None or self._scratch.numel() < need:
             self._scratch = self._torch.empty(need, dtype=self._torch.uint8, device=self.device)
@@ -220,7 +238,7 @@ class DeviceActor(_NetworkSource):
             raise ValueError("observation width %d is not selectedAction * 5 + 9 + 1024; supported: %s" % (state.shape[1], SUPPORTED))
         return state if state.stride(1) == 1 else state.contiguous(), width // 5
 
-    def _run(self, state, mask, shape_feature, want_q):
+    def _inputs(self, state, shape_feature):
         torch = self._torch
         state, sel = self._check_state(state)
         N = state.shape[0]
@@ -236,6 +254,12 @@ class DeviceActor(_NetworkSource):
                 or tuple(shape_feature.shape) != (N, EMB)):
             raise ValueError("shape_feature must be a tensor [%d, %d] on %s" % (N, EMB, self.device))
         shape_feature = shape_feature.detach().to(torch.float32).contiguous()
+        w = _lib.IrbppDqnWeights(*([ws[f].data_ptr() for f, _ in _FIELDS] + [ctypes.c_float(0.01)]))
+        return state, sel, N, ws, enc, shape_feature, w
+
+    def _run(self, state, mask, shape_feature, want_q):
+        torch = self._torch
+        state, sel, N, ws, enc, shape_feature, w = self._inputs(state, shape_feature)
         m_ptr, m_row, m_elem = 0, 0, 0
         if mask is not None:
             if not isinstance(mask, torch.Tensor) or mask.device != self.device or tuple(mask.shape) != (N, sel):
@@ -246,7 +270,6 @@ class DeviceActor(_NetworkSource):
         self._scratch_of(int(self._lib.irbpp_dqn_scratch_bytes(N, sel)))
         actions = torch.empty(N, dtype=torch.int64, device=self.device)
         q = torch.empty((N, sel), dtype=torch.float32, device=self.device) if want_q else None
-        w = _lib.IrbppDqnWeights(*([ws[f].data_ptr() for f, _ in _FIELDS] + [ctypes.c_float(0.01)]))
         rc = self._lib.irbpp_dqn_act(ctypes.byref(w), state.data_ptr(), state.stride(0), N, sel, shape_feature.data_ptr(),
                                      self.support.data_ptr(), self.atoms, m_ptr, m_row, m_elem, actions.data_ptr(),
                                      q.data_ptr() if q is not None else 0, self._scratch.data_ptr(), self._scratch.numel(),
@@ -263,6 +286,28 @@ class DeviceActor(_NetworkSource):
     def q_values(self, state, mask=None, shape_feature=None):
         """The masked ``sum_q_map`` of agent.py:53-57: float32 ``[N, sel]`` (-inf where ``mask != 1``)."""
         return self._run(state, mask, shape_feature, True)[1]
+
+    def target(self, next_state, next_actions, returns, nonterminals, v_min, v_max, discount_n, shape_feature=None,
+               with_p=True):
+        """The target distribution of ``Agent.learn`` (agent.py:94-115) through ``irbpp_dqn_target``, with this actor's
+        network as the target net: ``p_next = p(s', a*)`` and ``m``, the projection of ``returns + nonterminals *
+        discount_n * z`` onto the support, both float32 ``[B, atoms]`` on the device.  ``next_actions``: a* of the
+        online net (``online_actor.act(next_state)``, unmasked as agent.py:90-92), clamped to the rows;
+        ``returns`` ``[B]`` and ``nonterminals`` ``[B, 1]`` as ``PrioritizedReplayBank.sample`` returns them.
+        ``with_p=False`` skips ``p_next`` (returned as None)."""
+        torch = self._torch
+        state, sel, B, ws, enc, shape_feature, w = self._inputs(next_state, shape_feature)
+        a, r, nt, m, p = self._target_inputs(B, next_actions, returns, nonterminals, v_min, v_max, with_p)
+        p_ptr = p.data_ptr() if p is not None else None
+        self._scratch_of(int(self._lib.irbpp_dqn_scratch_bytes(B, sel)))
+        rc = self._lib.irbpp_dqn_target(ctypes.byref(w), state.data_ptr(), state.stride(0), B, sel, shape_feature.data_ptr(),
+                                        self.support.data_ptr(), self.atoms, a.data_ptr(), r.data_ptr(), nt.data_ptr(),
+                                        float(discount_n), float(v_min), float(v_max), m.data_ptr(), p_ptr,
+                                        self._scratch.data_ptr(), self._scratch.numel(),
+                                        torch.cuda.current_stream(self.device).cuda_stream)
+        _lib.check(self._lib, None, rc)
+        self._keep = (ws, enc, shape_feature, state, a, r, nt)
+        return m, p
 
 
 class DeviceOrderActor(_NetworkSource):
@@ -307,7 +352,7 @@ class DeviceOrderActor(_NetworkSource):
             raise ValueError("order observation width %d is not bufferSize + 1024; supported: %s" % (state.shape[1], ORDER_SUPPORTED))
         return state if state.stride(1) == 1 else state.contiguous(), k
 
-    def _run(self, state, mask, shape_features, want_q):
+    def _inputs(self, state, shape_features):
         torch = self._torch
         state, k = self._check_state(state)
         N = state.shape[0]
@@ -321,6 +366,12 @@ class DeviceOrderActor(_NetworkSource):
                 or shape_features.dim() != 2 or shape_features.shape[1] != EMB or shape_features.shape[0] < 1):
             raise ValueError("shape_features must be a tensor [S, %d] on %s" % (EMB, self.device))
         shape_features = shape_features.detach().to(torch.float32).contiguous()
+        w = _lib.IrbppDqnOrderWeights(*([ws[f].data_ptr() for f, _ in _ORDER_FIELDS] + [ctypes.c_float(0.01)]))
+        return state, k, N, ws, enc, shape_features, w
+
+    def _run(self, state, mask, shape_features, want_q):
+        torch = self._torch
+        state, k, N, ws, enc, shape_features, w = self._inputs(state, shape_features)
         S = shape_features.shape[0]
         m_ptr, m_row, m_elem = 0, 0, 0
         if mask is not None:
@@ -332,7 +383,6 @@ class DeviceOrderActor(_NetworkSource):
         scratch = self._scratch_of(int(self._lib.irbpp_dqn_order_scratch_bytes(N, k, S)))
         actions = torch.empty(N, dtype=torch.int64, device=self.device)
         q = torch.empty((N, k), dtype=torch.float32, device=self.device) if want_q else None
-        w = _lib.IrbppDqnOrderWeights(*([ws[f].data_ptr() for f, _ in _ORDER_FIELDS] + [ctypes.c_float(0.01)]))
         rc = self._lib.irbpp_dqn_order_act(ctypes.byref(w), state.data_ptr(), state.stride(0), N, k, shape_features.data_ptr(),
                                            S, self.support.data_ptr(), self.atoms, m_ptr, m_row, m_elem, actions.data_ptr(),
                                            q.data_ptr() if q is not None else 0, scratch.data_ptr(), scratch.numel(),
@@ -349,3 +399,22 @@ class DeviceOrderActor(_NetworkSource):
     def q_values(self, order_state, mask=None, shape_features=None):
         """The masked ``sum_q_map`` of agent.py:53-57: float32 ``[N, k]`` (-inf where ``mask != 1``)."""
         return self._run(order_state, mask, shape_features, True)[1]
+
+    def target(self, next_state, next_actions, returns, nonterminals, v_min, v_max, discount_n, shape_features=None,
+               with_p=True):
+        """``DeviceActor.target`` at the order level, through ``irbpp_dqn_order_target``: ``(m, p_next)`` for the
+        order network's ``learn`` (trainer.py:318), a* clamped to the k slots."""
+        torch = self._torch
+        state, k, B, ws, enc, shape_features, w = self._inputs(next_state, shape_features)
+        S = shape_features.shape[0]
+        a, r, nt, m, p = self._target_inputs(B, next_actions, returns, nonterminals, v_min, v_max, with_p)
+        p_ptr = p.data_ptr() if p is not None else None
+        scratch = self._scratch_of(int(self._lib.irbpp_dqn_order_scratch_bytes(B, k, S)))
+        rc = self._lib.irbpp_dqn_order_target(ctypes.byref(w), state.data_ptr(), state.stride(0), B, k,
+                                              shape_features.data_ptr(), S, self.support.data_ptr(), self.atoms,
+                                              a.data_ptr(), r.data_ptr(), nt.data_ptr(), float(discount_n), float(v_min),
+                                              float(v_max), m.data_ptr(), p_ptr, scratch.data_ptr(),
+                                              scratch.numel(), torch.cuda.current_stream(self.device).cuda_stream)
+        _lib.check(self._lib, None, rc)
+        self._keep = (ws, enc, shape_features, state, a, r, nt)
+        return m, p

@@ -1067,11 +1067,27 @@ int64_t irbpp_dqn_scratch_bytes(int32_t N, int32_t selected_action) {
     return actor_scratch_bytes(N, selected_action);
 }
 
-int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t selected_action,
-                  const float* shape_feature, const float* support, int32_t atoms, const float* mask, int64_t mask_row_stride,
-                  int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch, int64_t scratch_bytes,
-                  void* stream) {
-    if (!weights || !obs || !shape_feature || !support || !actions || !scratch) return fail(nullptr, IRBPP_EINVAL, "null act argument");
+// the arguments of Agent.learn's target pass beyond the act's (irbpp_dqn_target, irbpp_dqn_order_target)
+static int learn_target_args(LearnTarget& T, int32_t atoms, const int64_t* next_actions, const float* returns,
+                             const float* nonterminals, double discount_n, double v_min, double v_max, float* m,
+                             float* p_next) {
+    if (!next_actions || !returns || !nonterminals || !m) return fail(nullptr, IRBPP_EINVAL, "null target argument");
+    if (atoms < 2 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [2, %d]", atoms, AC_MAXATOMS);
+    if (!(v_max > v_min)) return fail(nullptr, IRBPP_EINVAL, "need v_max > v_min (v_min %g, v_max %g)", v_min, v_max);
+    const double dz = (v_max - v_min) / (atoms - 1);           // agent.py:20, in double
+    T.next_actions = next_actions; T.returns = returns; T.nonterminals = nonterminals;
+    T.gamma_n = (float)discount_n; T.v_min = (float)v_min; T.v_max = (float)v_max;
+    T.inv_dz = 1.0f / (float)dz;                                 // torch's CUDA tensor / scalar (irbpp_learn.cuh)
+    T.m = m; T.p_next = p_next;
+    return IRBPP_OK;
+}
+
+// irbpp_dqn_act (T == NULL) and irbpp_dqn_target (T: the target mode's arguments, checked)
+static int dqn_forward(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t N,
+                       int32_t selected_action, const float* shape_feature, const float* support, int32_t atoms,
+                       const float* mask, int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions,
+                       float* sum_q_map, void* scratch, int64_t scratch_bytes, void* stream, const LearnTarget* T) {
+    if (!weights || !obs || !shape_feature || !support || (!T && !actions) || !scratch) return fail(nullptr, IRBPP_EINVAL, "null act argument");
     if (N <= 0 || selected_action <= 0) return fail(nullptr, IRBPP_EINVAL, "need N >= 1 bins and selected_action >= 1 (N %d, sel %d)", N, selected_action);
     if (atoms < 1 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [1, %d]", atoms, AC_MAXATOMS);
     if (obs_stride < (int64_t)selected_action * 5 + 9 + AC_HM * AC_HM)
@@ -1097,12 +1113,34 @@ int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t ob
     actor_scratch_layout(A, scratch);
     const int dev = device_of(obs);
     DeviceGuard guard(dev);
-    cudaError_t e = raise_dynamic_smem(dev, (const void*)irbpp_actor_rows_kernel, AC_ROWS_SMEM_BYTES);
+    const void* rows = T ? (const void*)irbpp_actor_target_kernel : (const void*)irbpp_actor_rows_kernel;
+    cudaError_t e = raise_dynamic_smem(dev, rows, AC_ROWS_SMEM_BYTES);
     if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "rows kernel set-up: %s", cudaGetErrorString(e));
     cudaStream_t s = (cudaStream_t)stream;
     irbpp_actor_bin_kernel<<<N, AC_THREADS, 0, s>>>(A);
-    irbpp_actor_rows_kernel<<<N, AC_THREADS, AC_ROWS_SMEM_BYTES, s>>>(A);
+    if (T) irbpp_actor_target_kernel<<<N, AC_THREADS, AC_ROWS_SMEM_BYTES, s>>>(A, *T);
+    else irbpp_actor_rows_kernel<<<N, AC_THREADS, AC_ROWS_SMEM_BYTES, s>>>(A);
     return launch_status();
+}
+
+int irbpp_dqn_act(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t selected_action,
+                  const float* shape_feature, const float* support, int32_t atoms, const float* mask, int64_t mask_row_stride,
+                  int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch, int64_t scratch_bytes,
+                  void* stream) {
+    return dqn_forward(weights, obs, obs_stride, N, selected_action, shape_feature, support, atoms, mask, mask_row_stride,
+                       mask_elem_stride, actions, sum_q_map, scratch, scratch_bytes, stream, nullptr);
+}
+
+int irbpp_dqn_target(const irbpp_dqn_weights* target, const float* next_obs, int64_t obs_stride, int32_t B,
+                     int32_t selected_action, const float* shape_feature, const float* support, int32_t atoms,
+                     const int64_t* next_actions, const float* returns, const float* nonterminals, double discount_n,
+                     double v_min, double v_max, float* m, float* p_next, void* scratch, int64_t scratch_bytes,
+                     void* stream) {
+    LearnTarget T;
+    const int rc = learn_target_args(T, atoms, next_actions, returns, nonterminals, discount_n, v_min, v_max, m, p_next);
+    if (rc) return rc;
+    return dqn_forward(target, next_obs, obs_stride, B, selected_action, shape_feature, support, atoms, nullptr, 0, 0,
+                       nullptr, nullptr, scratch, scratch_bytes, stream, &T);
 }
 
 // ---- the order network's forward pass and Agent.act (csrc/irbpp_order_actor.cuh) ---------------------------------
@@ -1111,11 +1149,12 @@ int64_t irbpp_dqn_order_scratch_bytes(int32_t N, int32_t k, int32_t S) {
     return order_scratch_bytes(N, S);
 }
 
-int irbpp_dqn_order_act(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t k,
-                        const float* shape_features, int32_t S, const float* support, int32_t atoms, const float* mask,
-                        int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch,
-                        int64_t scratch_bytes, void* stream) {
-    if (!weights || !obs || !shape_features || !support || !actions || !scratch) return fail(nullptr, IRBPP_EINVAL, "null order act argument");
+// irbpp_dqn_order_act (T == NULL) and irbpp_dqn_order_target (T: the target mode's arguments, checked)
+static int dqn_order_forward(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t N,
+                             int32_t k, const float* shape_features, int32_t S, const float* support, int32_t atoms,
+                             const float* mask, int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions,
+                             float* sum_q_map, void* scratch, int64_t scratch_bytes, void* stream, const LearnTarget* T) {
+    if (!weights || !obs || !shape_features || !support || (!T && !actions) || !scratch) return fail(nullptr, IRBPP_EINVAL, "null order act argument");
     if (N <= 0 || S <= 0) return fail(nullptr, IRBPP_EINVAL, "need N >= 1 bins and S >= 1 shapes (N %d, S %d)", N, S);
     if (k < 2 || k > OA_MAXK) return fail(nullptr, IRBPP_EINVAL, "buffer size k %d outside [2, %d]", k, OA_MAXK);
     if (atoms < 1 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [1, %d]", atoms, AC_MAXATOMS);
@@ -1142,14 +1181,36 @@ int irbpp_dqn_order_act(const irbpp_dqn_order_weights* weights, const float* obs
     order_scratch_layout(A, scratch);
     const int dev = device_of(obs);
     DeviceGuard guard(dev);
-    cudaError_t e = raise_dynamic_smem(dev, (const void*)irbpp_order_slots_kernel, OA_SLOTS_SMEM_BYTES);
+    const void* slots = T ? (const void*)irbpp_order_target_kernel : (const void*)irbpp_order_slots_kernel;
+    cudaError_t e = raise_dynamic_smem(dev, slots, OA_SLOTS_SMEM_BYTES);
     if (e != cudaSuccess) return fail(nullptr, IRBPP_ECUDA, "slots kernel set-up: %s", cudaGetErrorString(e));
     cudaStream_t s = (cudaStream_t)stream;
     const int per = AC_TM / k;
     irbpp_order_table_kernel<<<S, AC_THREADS, 0, s>>>(A);
     irbpp_order_bin_kernel<<<N, AC_THREADS, 0, s>>>(A);
-    irbpp_order_slots_kernel<<<(N + per - 1) / per, AC_THREADS, OA_SLOTS_SMEM_BYTES, s>>>(A);
+    if (T) irbpp_order_target_kernel<<<(N + per - 1) / per, AC_THREADS, OA_SLOTS_SMEM_BYTES, s>>>(A, *T);
+    else irbpp_order_slots_kernel<<<(N + per - 1) / per, AC_THREADS, OA_SLOTS_SMEM_BYTES, s>>>(A);
     return launch_status();
+}
+
+int irbpp_dqn_order_act(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t N, int32_t k,
+                        const float* shape_features, int32_t S, const float* support, int32_t atoms, const float* mask,
+                        int64_t mask_row_stride, int64_t mask_elem_stride, int64_t* actions, float* sum_q_map, void* scratch,
+                        int64_t scratch_bytes, void* stream) {
+    return dqn_order_forward(weights, obs, obs_stride, N, k, shape_features, S, support, atoms, mask, mask_row_stride,
+                             mask_elem_stride, actions, sum_q_map, scratch, scratch_bytes, stream, nullptr);
+}
+
+int irbpp_dqn_order_target(const irbpp_dqn_order_weights* target, const float* next_obs, int64_t obs_stride, int32_t B,
+                           int32_t k, const float* shape_features, int32_t S, const float* support, int32_t atoms,
+                           const int64_t* next_actions, const float* returns, const float* nonterminals,
+                           double discount_n, double v_min, double v_max, float* m, float* p_next, void* scratch,
+                           int64_t scratch_bytes, void* stream) {
+    LearnTarget T;
+    const int rc = learn_target_args(T, atoms, next_actions, returns, nonterminals, discount_n, v_min, v_max, m, p_next);
+    if (rc) return rc;
+    return dqn_order_forward(target, next_obs, obs_stride, B, k, shape_features, S, support, atoms, nullptr, 0, 0,
+                             nullptr, nullptr, scratch, scratch_bytes, stream, &T);
 }
 
 int irbpp_debug_phase_cycles(irbpp_handle h, int32_t enable, uint64_t* out8) {

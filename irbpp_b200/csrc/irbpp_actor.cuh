@@ -20,6 +20,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "irbpp_learn.cuh"
+
 namespace irbpp {
 
 constexpr int AC_THREADS = 256;            // both kernels
@@ -310,7 +312,10 @@ __global__ void __launch_bounds__(AC_THREADS) irbpp_actor_bin_kernel(const Actor
 //   -> fc_h_a 128 (ReLU) -> fc_z_a atoms = advantages (stored by row index in the scratch, summed for mean(a)),
 // then the final phase: value head on g = sum / sel, mean(a) = (sum_valid a + (sel - n_valid) a0) / sel,
 // q = v + a - mean(a) (a0 for invalid rows), softmax over the atoms, expectation over the support, mask, argmax.
-__global__ void __launch_bounds__(AC_THREADS, 2) irbpp_actor_rows_kernel(const ActorParams A) {
+// TARGET (irbpp_actor_target_kernel): the final phase instead builds p = softmax(q) of row a* = T.next_actions[b] only
+// and projects it (learn_project); no expectation, argmax or sum_q.
+template <bool TARGET>
+__device__ __forceinline__ void actor_rows(const ActorParams A, const LearnTarget& T) {
     extern __shared__ __align__(16) float ac_smem[];
     float* P = ac_smem;                               // [AC_TM][AC_LD_P]
     float* Q = P + AC_TM * AC_LD_P;                   // [AC_TM][AC_LD_Q]
@@ -406,6 +411,25 @@ __global__ void __launch_bounds__(AC_THREADS, 2) irbpp_actor_rows_kernel(const A
     __syncthreads();
     if (tid < AC_MAXATOMS) base[tid] = (asum[tid] + (float)(sel - nv) * a0[tid]) / (float)sel;   // mean(a) over all rows
     __syncthreads();
+    if constexpr (TARGET) {                                                 // warp 0, lane = atom, row a*
+        if (warp != 0) return;
+        int64_t r = T.next_actions[b];
+        r = r < 0 ? 0 : (r >= sel ? sel - 1 : r);
+        const bool valid = ob[r * 5 + 4] == 1.0f;
+        const float az = valid ? adv[r * AC_MAXATOMS + lane] : a0[lane];
+        const float qz = lane < atoms ? (v[lane] + az) - base[lane] : -INFINITY;
+        float m = qz;
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, s));
+        const float e = lane < atoms ? expf(qz - m) : 0.0f;
+        float se = e;
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) se += __shfl_xor_sync(0xffffffffu, se, s);
+        const float p = e / se;
+        if (T.p_next && lane < atoms) T.p_next[(int64_t)b * atoms + lane] = p;
+        learn_project(T, b, atoms, p, lane < atoms ? A.support[lane] : 0.0f, lane);
+        return;
+    }
     // one warp per row, lane = atom
     const float sup = lane < atoms ? A.support[lane] : 0.0f;
     const float vz = v[lane], mz = base[lane], a0z = a0[lane];      // lanes >= atoms hold zeros
@@ -438,6 +462,15 @@ __global__ void __launch_bounds__(AC_THREADS, 2) irbpp_actor_rows_kernel(const A
             if (wbest[w] > bb || (wbest[w] == bb && wbidx[w] < bi)) { bb = wbest[w]; bi = wbidx[w]; }
         A.actions[b] = bi < sel ? bi : 0;
     }
+}
+
+__global__ void __launch_bounds__(AC_THREADS, 2) irbpp_actor_rows_kernel(const ActorParams A) {
+    actor_rows<false>(A, LearnTarget{});
+}
+
+// Agent.learn's target pass (agent.py:94-115) over the target net: irbpp_dqn_target
+__global__ void __launch_bounds__(AC_THREADS, 2) irbpp_actor_target_kernel(const ActorParams A, const LearnTarget T) {
+    actor_rows<true>(A, T);
 }
 
 }  // namespace irbpp

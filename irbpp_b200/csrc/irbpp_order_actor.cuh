@@ -112,7 +112,10 @@ __global__ void __launch_bounds__(AC_THREADS) irbpp_order_bin_kernel(const Order
 //   X[lb] = mean_j H[lb * k + j] (g, model.py:381-382); P[:, 0:128] = relu(fc_h_v(X)); P[:, 128:160] = fc_z_v(...) = v
 //   X = relu(fc_h_a(H)); P[:, 160:192] = fc_z_a(X) = a;  S[lb] = mean_j a
 //   q = v + a - mean(a), softmax over the atoms, expectation over the support, mask, argmax over the k slots.
-__global__ void __launch_bounds__(AC_THREADS, 1) irbpp_order_slots_kernel(const OrderParams A) {
+// TARGET (irbpp_order_target_kernel): the final phase instead builds p = softmax(q) of slot a* = T.next_actions[b] of
+// each bin only, one warp per bin, and projects it (learn_project, irbpp_learn.cuh); no expectation, argmax or sum_q.
+template <bool TARGET>
+__device__ __forceinline__ void order_slots(const OrderParams A, const LearnTarget& T) {
     extern __shared__ __align__(16) float oa_smem[];
     float* H = oa_smem;                               // [AC_TM][AC_LD_Q]
     float* X = H + AC_TM * AC_LD_Q;                   // [AC_TM][AC_LD_Q]
@@ -214,6 +217,27 @@ __global__ void __launch_bounds__(AC_THREADS, 1) irbpp_order_slots_kernel(const 
     __syncthreads();
     // one warp per row, lane = atom
     const float sup = lane < atoms ? A.support[lane] : 0.0f;
+    if constexpr (TARGET) {                                     // one warp per bin, slot a*
+        for (int lb = warp; lb < nb; lb += AC_THREADS / 32) {
+            const int64_t b = b0 + lb;
+            int64_t j = T.next_actions[b];
+            j = j < 0 ? 0 : (j >= k ? k - 1 : j);
+            const int r = lb * k + (int)j;
+            const float qz = lane < atoms ? (P[lb * AC_LD_P + AC_EMB + lane] + P[r * AC_LD_P + AC_EMB + 32 + lane]) - S[lb * 32 + lane]
+                                          : -INFINITY;
+            float m = qz;
+#pragma unroll
+            for (int s = 16; s > 0; s >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, s));
+            const float e = lane < atoms ? expf(qz - m) : 0.0f;
+            float se = e;
+#pragma unroll
+            for (int s = 16; s > 0; s >>= 1) se += __shfl_xor_sync(0xffffffffu, se, s);
+            const float p = e / se;
+            if (T.p_next && lane < atoms) T.p_next[b * atoms + lane] = p;
+            learn_project(T, b, atoms, p, sup, lane);
+        }
+        return;
+    }
     for (int r = warp; r < nr; r += AC_THREADS / 32) {
         const int lb = r / k, j = r - lb * k, b = b0 + lb;
         const float qz = lane < atoms ? (P[lb * AC_LD_P + AC_EMB + lane] + P[r * AC_LD_P + AC_EMB + 32 + lane]) - S[lb * 32 + lane]
@@ -242,6 +266,15 @@ __global__ void __launch_bounds__(AC_THREADS, 1) irbpp_order_slots_kernel(const 
             if (sq[tid * k + j] > best) { best = sq[tid * k + j]; bi = j; }
         A.actions[b0 + tid] = bi;
     }
+}
+
+__global__ void __launch_bounds__(AC_THREADS, 1) irbpp_order_slots_kernel(const OrderParams A) {
+    order_slots<false>(A, LearnTarget{});
+}
+
+// Agent.learn's target pass (agent.py:94-115) over the order-level target net: irbpp_dqn_order_target
+__global__ void __launch_bounds__(AC_THREADS, 1) irbpp_order_target_kernel(const OrderParams A, const LearnTarget T) {
+    order_slots<true>(A, T);
 }
 
 }  // namespace irbpp

@@ -16,6 +16,8 @@ iteration rate.  This module keeps the loop's shape and removes the per-environm
 * ``segment_size``         -- the shim for ``agent.py:69``;
 * ``PrioritizedReplayBank`` -- the reference's replay itself (``memory.py``: float32 sum tree, n-step returns,
   importance weights, stratified draws) for N memories on the device (``csrc/irbpp_replay.cuh``).
+* ``device_learn``         -- ``Agent.learn`` (``agent.py:68-125``) with its two no-grad passes on the device
+  (``DeviceActor.act`` / ``.target``); the gradient pass, the backward pass and the optimiser stay in torch.
 
 ``ReplayBank`` samples uniformly; it exists so that the actor loop can be run end to end at N = 4096 and timed
 (``tools/actor_loop.py``).
@@ -296,3 +298,41 @@ class PrioritizedReplayBank(object):
             self._call(self._lib.irbpp_replay_update_priorities(
                 self._ctypes.byref(self._mem), mids.data_ptr(), idx.data_ptr(), loss.data_ptr(), idx.numel(),
                 self.priority_exponent, self._flags.data_ptr(), self._stream()))
+
+
+def device_learn(agent, bank, online_actor, target_actor):
+    """``agent.learn(mem)`` (``agent.py:68-125``) on a ``PrioritizedReplayBank``, for either network level (the level
+    follows from the actors): ``online_actor`` wraps ``agent.online_net`` and ``target_actor`` wraps
+    ``agent.target_net`` (both ``DeviceActor`` or both ``DeviceOrderActor``, read live).  Returns the loss ``[B]`` on
+    the device.  The calls keep the reference's order, so torch's RNG is consumed as the reference consumes it:
+
+    1. ``bank.sample(agent.batch_size)``;
+    2. ``agent.online_net(states, log=True)`` with gradients (agent.py:85-86);
+    3. ``online_actor.act(next_states)``, unmasked: the double-Q a* (agent.py:90-92);
+    4. ``agent.target_net.reset_noise()`` (agent.py:94);
+    5. ``target_actor.target(...)``: p(s', a*; target) and its projection m (agent.py:96-115);
+    6. the loss, the importance-weighted mean, ``backward``, ``clip_grad_norm_`` and ``optimiser.step()`` exactly as
+       agent.py:117-121;
+    7. ``bank.update_priorities`` with the loss (agent.py:123-124).
+
+    One difference from the reference: its three forward passes each draw point indices with ``np.random``
+    (model.py:331, 367); here only the gradient pass does, and the two device passes draw from the counter-based
+    generator of their actors' ``DeviceShapeClouds`` / ``OrderShapeClouds``, one index set per net."""
+    import torch
+    from torch.nn.utils import clip_grad_norm_
+    idxs, states, actions, returns, next_states, nonterminals, weights, mem_ids = bank.sample(agent.batch_size)
+    B = states.shape[0]
+    log_ps = agent.online_net(states, log=True)
+    log_ps_a = log_ps[torch.arange(B, device=log_ps.device), actions]
+    with torch.no_grad():
+        next_actions = online_actor.act(next_states)
+        agent.target_net.reset_noise()
+        m, _ = target_actor.target(next_states, next_actions, returns, nonterminals, agent.Vmin, agent.Vmax,
+                                   agent.discount ** agent.n, with_p=False)
+    loss = -torch.sum(m * log_ps_a, 1)
+    agent.online_net.zero_grad()
+    (weights * loss).mean().backward()
+    clip_grad_norm_(agent.online_net.parameters(), agent.norm_clip)
+    agent.optimiser.step()
+    bank.update_priorities(idxs, mem_ids, loss.detach())
+    return loss
