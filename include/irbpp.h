@@ -418,6 +418,51 @@ int irbpp_dqn_order_target(const irbpp_dqn_order_weights* target, const float* n
                            double discount_n, double v_min, double v_max, float* m, float* p_next, void* scratch,
                            int64_t scratch_bytes, void* stream);
 
+/* ---- the gradient pass of Agent.learn at the location level (csrc/irbpp_grad.cuh) -----------------------------------
+ * The candidate-row network of DQNBPP (bufferSize == 1) from its inputs to log p(s, a_t, .) (agent.py:85-86 with
+ * model.py:316-352, 386-404), and its backward pass.  The caller computes, with autograd, shape_feature [B, 128]
+ * (shapeEncoder, max over the points) and map_feature [B, 256] (heightEncoder), and the NoisyLinear effective weights;
+ * the kernels take them as inputs and return their gradients.  Handle-free, like irbpp_dqn_act, with its weight
+ * conventions; the heightEncoder fields of irbpp_dqn_weights are not read and may be NULL.  Supported: hidden_size 128,
+ * 1 <= atoms <= 32, selected_action >= 1, B * (selected_action + 1) < 2^31.  An action outside [0, selected_action) is
+ * clamped into it (the reference raises IndexError there).  Float32 throughout, no atomics: two calls on the same
+ * inputs give bit-identical results. */
+
+/* Gradients of the effective row-section tensors, one float32 device output per row-section field of
+ * irbpp_dqn_weights, each in that field's layout. */
+typedef struct {
+    float* cand1_w; float* cand1_b;     /* init_candidate_embed.0 [32, 4], [32] */
+    float* cand2_w; float* cand2_b;     /* init_candidate_embed.2 [128, 32], [128] */
+    float* proj1_w; float* proj1_b;     /* project_layer.0 [256, 512], [256] */
+    float* proj2_w; float* proj2_b;     /* project_layer.2 [128, 256], [128] */
+    float* fc_h_v_w; float* fc_h_v_b;   /* fc_h_v [128, 128], [128] */
+    float* fc_z_v_w; float* fc_z_v_b;   /* fc_z_v [atoms, 128], [atoms] */
+    float* fc_h_a_w; float* fc_h_a_b;   /* fc_h_a [128, 128], [128] */
+    float* fc_z_a_w; float* fc_z_a_b;   /* fc_z_a [atoms, 128], [atoms] */
+} irbpp_dqn_grads;
+
+/* Bytes of the scratch irbpp_dqn_log_prob and irbpp_dqn_log_prob_backward need for B transitions of selected_action
+ * rows (-1 for bad sizes). */
+int64_t irbpp_dqn_log_prob_scratch_bytes(int32_t B, int32_t selected_action);
+
+/* obs float32 [B] rows of obs_stride >= selected_action * 5 + 9 + 1024 (the sampled states; column 4 of the candidate
+ * rows is the mask whose rows model.py:347-349 zeroes), shape_feature float32 [B, 128], map_feature float32 [B, 256],
+ * actions int64 [B] (a_t).  Writes log_p float32 [B, atoms] = log_softmax(q(s, a_t)) computed as
+ * q - max - log sum exp(q - max).  scratch: irbpp_dqn_log_prob_scratch_bytes bytes, 256-byte aligned. */
+int irbpp_dqn_log_prob(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                       int32_t selected_action, const float* shape_feature, const float* map_feature,
+                       const int64_t* actions, int32_t atoms, float* log_p, void* scratch, int64_t scratch_bytes,
+                       void* stream);
+
+/* The backward pass of irbpp_dqn_log_prob on the same inputs: given grad_log_p float32 [B, atoms] = dL/dlog_p, writes
+ * dL/d(tensor) for every tensor of grads (overwritten, not accumulated), d_shape_feature float32 [B, 128] and
+ * d_map_feature float32 [B, 256].  The forward pass is recomputed inside the call; the scratch is the forward's size. */
+int irbpp_dqn_log_prob_backward(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                                int32_t selected_action, const float* shape_feature, const float* map_feature,
+                                const int64_t* actions, int32_t atoms, const float* grad_log_p,
+                                const irbpp_dqn_grads* grads, float* d_shape_feature, float* d_map_feature,
+                                void* scratch, int64_t scratch_bytes, void* stream);
+
 /* Profiling aid: when enabled, thread 0 of every CTA adds the SM cycles it spent in each kernel phase
  * (0 scan kernel: load + apply action, 1 scan kernel: observation heightmap + scan + level bitmaps,
  * 2 candidates kernel: contour tasks, 3 candidates kernel: select / pad) to counters 0-3; counters 4-7 count

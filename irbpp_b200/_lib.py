@@ -61,6 +61,13 @@ class IrbppDqnOrderWeights(ctypes.Structure):
                                          "fc_h_a_b", "fc_z_a_w", "fc_z_a_b")] + [("negative_slope", ctypes.c_float)]
 
 
+class IrbppDqnGrads(ctypes.Structure):
+    """``irbpp_dqn_grads``: device pointers of the gradients of the location network's row-section tensors."""
+    _fields_ = [(n, c_void_p) for n in ("cand1_w", "cand1_b", "cand2_w", "cand2_b", "proj1_w", "proj1_b", "proj2_w",
+                                         "proj2_b", "fc_h_v_w", "fc_h_v_b", "fc_z_v_w", "fc_z_v_b", "fc_h_a_w", "fc_h_a_b",
+                                         "fc_z_a_w", "fc_z_a_b")]
+
+
 # symbol -> (restype, argtypes); every symbol of include/irbpp.h appears here (checked by the tests)
 SIGNATURES = {
     "irbpp_abi_version": (c_i32, []),
@@ -108,6 +115,12 @@ SIGNATURES = {
     "irbpp_dqn_order_target": (c_i32, [ctypes.POINTER(IrbppDqnOrderWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_i32,
                                        c_void_p, c_i32, c_void_p, c_void_p, c_void_p, c_f64, c_f64, c_f64, c_void_p,
                                        c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_dqn_log_prob_scratch_bytes": (c_i64, [c_i32, c_i32]),
+    "irbpp_dqn_log_prob": (c_i32, [ctypes.POINTER(IrbppDqnWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p, c_void_p,
+                                   c_void_p, c_i32, c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_dqn_log_prob_backward": (c_i32, [ctypes.POINTER(IrbppDqnWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p,
+                                            c_void_p, c_void_p, c_i32, c_void_p, ctypes.POINTER(IrbppDqnGrads), c_void_p,
+                                            c_void_p, c_void_p, c_i64, c_void_p]),
     "irbpp_replay_init": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p]),
     "irbpp_replay_append": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
                                     c_void_p, ctypes.c_float, c_void_p]),

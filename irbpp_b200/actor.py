@@ -309,6 +309,102 @@ class DeviceActor(_NetworkSource):
         self._keep = (ws, enc, shape_feature, state, a, r, nt)
         return m, p
 
+    def log_prob(self, states, actions):
+        """``online_net(states, log=True)[arange(B), actions]`` of ``Agent.learn``'s gradient pass (agent.py:85-86):
+        float32 ``[B, atoms]``, differentiable with respect to every parameter of the live module the forward pass uses.
+        torch computes the height encoder, the shape encoder on ``clouds.sample(states)`` and the NoisyLinear effective
+        weights with autograd; ``irbpp_dqn_log_prob`` / ``irbpp_dqn_log_prob_backward`` run the candidate-row network
+        and its backward pass.  ``actions`` (a_t, ``[B]``) are clamped to the rows, where the reference raises
+        ``IndexError``.  Double backward is not supported."""
+        torch = self._torch
+        if self.net is None:
+            raise ValueError("log_prob trains the live module; a state-dict actor has no parameters")
+        state, sel = self._check_state(states)
+        B = state.shape[0]
+        if not isinstance(actions, torch.Tensor) or actions.device != self.device or actions.numel() != B:
+            raise ValueError("actions must be a tensor of %d values on %s" % (B, self.device))
+        if self.clouds is None:
+            raise ValueError("log_prob samples the next item's points: the actor needs a DeviceShapeClouds")
+        if self.clouds.item_col != sel * 5:
+            raise ValueError("the point clouds read the item id at column %d, the observation carries it at %d"
+                             % (self.clouds.item_col, sel * 5))
+        self._state()                                            # the weights' device
+        net = self.net
+        params = dict(net.named_parameters())
+        params.update(net.named_buffers())
+        eff = {}
+        for m in NOISY:                                          # model.py:224-228, with autograd
+            if net.training:
+                eff[m + ".weight"] = params[m + ".weight_mu"] + params[m + ".weight_sigma"] * params[m + ".weight_epsilon"]
+                eff[m + ".bias"] = params[m + ".bias_mu"] + params[m + ".bias_sigma"] * params[m + ".bias_epsilon"]
+            else:
+                eff[m + ".weight"], eff[m + ".bias"] = params[m + ".weight_mu"], params[m + ".bias_mu"]
+        weights = [(eff[k] if k in eff else params[k]).to(torch.float32).contiguous() for _, k in _ROW_FIELDS]
+        hm = state[:, sel * 5 + 9:sel * 5 + 9 + HM * HM].reshape(B, 1, HM, HM)
+        map_feature = net.heightEncoder(hm).reshape(B, -1)                            # model.py:326-327
+        shape_feature = net.shapeEncoder(self.clouds.sample(state)).max(1)[0]          # model.py:329-335
+        a = actions.detach().reshape(B).to(torch.int64).contiguous()
+        return _log_prob_function().apply(self, state, sel, a, shape_feature.to(torch.float32).contiguous(),
+                                          map_feature.to(torch.float32).contiguous(), *weights)
+
+
+# the row-section fields of irbpp_dqn_weights: the tensors irbpp_dqn_log_prob reads and irbpp_dqn_grads returns
+_ROW_FIELDS = _FIELDS[6:]
+_LOG_PROB = []
+
+
+def _log_prob_function():
+    """The ``torch.autograd.Function`` behind ``DeviceActor.log_prob`` (built once; torch is imported lazily here)."""
+    if _LOG_PROB:
+        return _LOG_PROB[0]
+    import torch
+
+    def weights_struct(ws):
+        ptrs = dict((f, t.data_ptr()) for (f, _), t in zip(_ROW_FIELDS, ws))
+        return _lib.IrbppDqnWeights(*([ptrs.get(f, 0) for f, _ in _FIELDS] + [ctypes.c_float(0.01)]))
+
+    class LogProb(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, actor, state, sel, actions, shape_feature, map_feature, *ws):
+            B = state.shape[0]
+            lib = actor._lib
+            w = weights_struct(ws)
+            scratch = actor._scratch_of(int(lib.irbpp_dqn_log_prob_scratch_bytes(B, sel)))
+            log_p = torch.empty((B, actor.atoms), dtype=torch.float32, device=actor.device)
+            rc = lib.irbpp_dqn_log_prob(ctypes.byref(w), state.data_ptr(), state.stride(0), B, sel,
+                                        shape_feature.data_ptr(), map_feature.data_ptr(), actions.data_ptr(), actor.atoms,
+                                        log_p.data_ptr(), scratch.data_ptr(), scratch.numel(),
+                                        torch.cuda.current_stream(actor.device).cuda_stream)
+            _lib.check(lib, None, rc)
+            ctx.actor, ctx.state, ctx.sel, ctx.actions = actor, state, sel, actions
+            ctx.save_for_backward(shape_feature, map_feature, *ws)
+            return log_p
+
+        @staticmethod
+        @torch.autograd.function.once_differentiable
+        def backward(ctx, grad):
+            actor, state, sel, actions = ctx.actor, ctx.state, ctx.sel, ctx.actions
+            shape_feature, map_feature = ctx.saved_tensors[:2]
+            ws = ctx.saved_tensors[2:]
+            B, lib = state.shape[0], actor._lib
+            grad = grad.to(torch.float32).contiguous()
+            w = weights_struct(ws)
+            dws = [torch.empty_like(t) for t in ws]
+            g = _lib.IrbppDqnGrads(*[t.data_ptr() for t in dws])
+            d_sf, d_mf = torch.empty_like(shape_feature), torch.empty_like(map_feature)
+            scratch = actor._scratch_of(int(lib.irbpp_dqn_log_prob_scratch_bytes(B, sel)))
+            rc = lib.irbpp_dqn_log_prob_backward(ctypes.byref(w), state.data_ptr(), state.stride(0), B, sel,
+                                                 shape_feature.data_ptr(), map_feature.data_ptr(), actions.data_ptr(),
+                                                 actor.atoms, grad.data_ptr(), ctypes.byref(g), d_sf.data_ptr(),
+                                                 d_mf.data_ptr(), scratch.data_ptr(), scratch.numel(),
+                                                 torch.cuda.current_stream(actor.device).cuda_stream)
+            _lib.check(lib, None, rc)
+            actor._keep = (grad, ws, state, actions)             # alive until the next call: the launches are asynchronous
+            return (None, None, None, None, d_sf, d_mf) + tuple(dws)
+
+    _LOG_PROB.append(LogProb)
+    return LogProb
+
 
 class DeviceOrderActor(_NetworkSource):
     """``Agent.act`` of the order network (``DQNBPP`` with ``args.level == 'order'``, ``bufferSize`` k > 1) for every

@@ -24,6 +24,7 @@
 #include "irbpp_replay.cuh"
 #include "irbpp_actor.cuh"
 #include "irbpp_order_actor.cuh"
+#include "irbpp_grad.cuh"
 
 using namespace irbpp;
 
@@ -1211,6 +1212,176 @@ int irbpp_dqn_order_target(const irbpp_dqn_order_weights* target, const float* n
     if (rc) return rc;
     return dqn_order_forward(target, next_obs, obs_stride, B, k, shape_features, S, support, atoms, nullptr, 0, 0,
                              nullptr, nullptr, scratch, scratch_bytes, stream, &T);
+}
+
+// ---- the gradient pass of Agent.learn at the location level (csrc/irbpp_grad.cuh) ---------------------------------
+int64_t irbpp_dqn_log_prob_scratch_bytes(int32_t B, int32_t selected_action) {
+    if (B <= 0 || selected_action <= 0 || (int64_t)B * (selected_action + 1) >= INT32_MAX) return -1;
+    return grad_scratch_bytes(B, selected_action);
+}
+
+// the argument checks both entry points share, and the parameter block
+static int grad_params(GradParams& P, const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                       int32_t sel, const float* shape_feature, const float* map_feature, const int64_t* actions,
+                       int32_t atoms, void* scratch, int64_t scratch_bytes) {
+    if (!weights || !obs || !shape_feature || !map_feature || !actions || !scratch)
+        return fail(nullptr, IRBPP_EINVAL, "null log-prob argument");
+    if (B <= 0 || sel <= 0) return fail(nullptr, IRBPP_EINVAL, "need B >= 1 transitions and selected_action >= 1 (B %d, sel %d)", B, sel);
+    if ((int64_t)B * (sel + 1) >= INT32_MAX) return fail(nullptr, IRBPP_EINVAL, "B * (selected_action + 1) too large (B %d, sel %d)", B, sel);
+    if (atoms < 1 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [1, %d]", atoms, AC_MAXATOMS);
+    if (obs_stride < (int64_t)sel * 5 + 9 + AC_HM * AC_HM)
+        return fail(nullptr, IRBPP_EINVAL, "observation stride %lld < selected_action * 5 + 9 + 1024", (long long)obs_stride);
+    if (scratch_bytes < grad_scratch_bytes(B, sel))
+        return fail(nullptr, IRBPP_EINVAL, "scratch of %lld bytes < %lld", (long long)scratch_bytes, (long long)grad_scratch_bytes(B, sel));
+    if (reinterpret_cast<uintptr_t>(scratch) & 255) return fail(nullptr, IRBPP_EINVAL, "scratch not 256-byte aligned");
+    const irbpp_dqn_weights& w = *weights;
+    const float* ptrs[] = {w.cand1_w, w.cand1_b, w.cand2_w, w.cand2_b, w.proj1_w, w.proj1_b, w.proj2_w, w.proj2_b, w.fc_h_v_w,
+                           w.fc_h_v_b, w.fc_z_v_w, w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b};
+    for (const float* p : ptrs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null weight pointer");
+    memset(&P, 0, sizeof(P));
+    P.w = ActorWeights{w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.cand1_w, w.cand1_b, w.cand2_w,
+                       w.cand2_b, w.proj1_w, w.proj1_b, w.proj2_w, w.proj2_b, w.fc_h_v_w, w.fc_h_v_b, w.fc_z_v_w,
+                       w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b, w.negative_slope};
+    P.obs = obs; P.obs_stride = obs_stride; P.B = B; P.sel = sel; P.atoms = atoms;
+    P.shape_feature = shape_feature; P.map_feature = map_feature; P.actions = actions;
+    grad_scratch_layout(P, scratch);
+    return IRBPP_OK;
+}
+
+// one GEMM of csrc/irbpp_grad.cuh: rows [row0, row0 + rows_host + *rows_dev), at most rows_max of them
+struct GradLauncher {
+    const GradParams& P;
+    cudaStream_t s;
+    int64_t cap;
+    GemmArgs base() const {
+        GemmArgs g;
+        memset(&g, 0, sizeof(g));
+        g.owner = P.owner; g.slope = P.w.slope;
+        return g;
+    }
+    // all rows (stand-ins and valid rows), the valid rows, the B transitions
+    void all(GemmArgs& g) const { g.row0 = 0; g.rows_host = P.B; g.rows_dev = P.count; }
+    void valid(GemmArgs& g) const { g.row0 = P.B; g.rows_host = 0; g.rows_dev = P.count; }
+    void per_transition(GemmArgs& g) const { g.row0 = 0; g.rows_host = P.B; g.rows_dev = nullptr; }
+    int64_t rows_max(const GemmArgs& g) const { return g.rows_host + (g.rows_dev ? (int64_t)P.B * P.sel : 0); }
+    int grid(int64_t tiles) const { return (int)std::max<int64_t>(1, std::min<int64_t>(tiles, cap)); }
+    // out[r][n] = act(in[r][:] . W[n][:] + bias[n] (+ add[owner r][n]))
+    void fwd(GemmArgs g, const float* in, int K, const float* W, int ldw, int N, const float* bias, float* out, int ldo,
+             int act, const float* add = nullptr, int ld_add = 0) const {
+        g.a = in; g.lda = K; g.b = W; g.ldb = ldw; g.c = out; g.ldc = ldo; g.bias = bias; g.add = add; g.ld_add = ld_add;
+        g.act = act; g.N = N; g.T = K;
+        irbpp_grad_fwd_kernel<<<grid((rows_max(g) + GR_TILE - 1) / GR_TILE * ((N + GR_TILE - 1) / GR_TILE)), GR_THREADS, 0, s>>>(g);
+    }
+    // out[r][k] = (dy[r][:] . W[:][k] (+ add[owner r][k])) * act'(out[r][k]) for k < K
+    void dgrad(GemmArgs g, const float* dy, int ldy, int N, const float* W, int ldw, int K, float* out, int ldo, int act,
+               const float* add = nullptr, int ld_add = 0) const {
+        g.a = dy; g.lda = ldy; g.b = W; g.ldb = ldw; g.c = out; g.ldc = ldo; g.add = add; g.ld_add = ld_add;
+        g.act = act; g.N = K; g.T = N;
+        irbpp_grad_dgrad_kernel<<<grid((rows_max(g) + GR_TILE - 1) / GR_TILE * ((K + GR_TILE - 1) / GR_TILE)), GR_THREADS, 0, s>>>(g);
+    }
+    // dW[n][k] (row stride ldo) = sum_r dy[r][n] x[r][k], db[n] = sum_r dy[r][n] (db may be NULL)
+    void wgrad(GemmArgs g, const float* dy, int ldy, int N, const float* x, int ldx, int K, float* dw, int ldo, float* db) const {
+        g.a = dy; g.lda = ldy; g.b = x; g.ldb = ldx; g.c = P.part; g.ldc = K; g.M = N; g.N = K;
+        const int64_t tiles = (int64_t)((N + GR_TILE - 1) / GR_TILE) * ((K + GR_TILE - 1) / GR_TILE) * GR_CHUNKS;
+        irbpp_grad_wgrad_kernel<<<grid(tiles), GR_THREADS, 0, s>>>(g);
+        irbpp_grad_reduce_kernel<<<grid(((int64_t)N * K + N + GR_THREADS - 1) / GR_THREADS), GR_THREADS, 0, s>>>(
+            P.part, N, K, K, dw, ldo, db);
+    }
+};
+
+// CTAs per GEMM launch: four per SM on the device.  The tile loop and the fixed row slices make the results independent
+// of the grid, so the host emulator, which runs CTAs one after another on 256 host threads each, takes one CTA.
+static int64_t grad_grid_cap(int dev) {
+#ifdef IRBPP_HOST_EMULATION
+    (void)dev; return 1;
+#else
+    return gather_grid_cap(dev) / 4;
+#endif
+}
+
+// the forward pass into the scratch; log_p written by the head when P.log_p is set
+static void grad_forward(const GradParams& P, const GradLauncher& L) {
+    const ActorWeights& w = P.w;
+    const int B = P.B;
+    irbpp_grad_prep_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    GemmArgs g = L.base();
+    L.per_transition(g);
+    L.fwd(g, P.xcat, 384, w.proj1_w, 512, AC_PROJ, w.proj1_b, P.u, AC_PROJ, ACT_NONE);            // u_b
+    irbpp_grad_scatter_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    L.valid(g);
+    L.fwd(g, P.cand, 4, w.cand1_w, 4, 32, w.cand1_b, P.h1, 32, ACT_LEAKY);                            // init_candidate_embed.0
+    L.fwd(g, P.h1, 32, w.cand2_w, 32, AC_EMB, w.cand2_b, P.ec, AC_EMB, ACT_NONE);                     // init_candidate_embed.2
+    L.fwd(g, P.ec, AC_EMB, w.proj1_w + 384, 512, AC_PROJ, nullptr, P.p0, AC_PROJ, ACT_LEAKY, P.u, AC_PROJ);  // project_layer.0
+    L.fwd(g, P.p0, AC_PROJ, w.proj2_w, AC_PROJ, AC_EMB, w.proj2_b, P.emb, AC_EMB, ACT_NONE);          // project_layer.2
+    L.all(g);
+    L.fwd(g, P.emb, AC_EMB, w.fc_h_a_w, AC_EMB, AC_EMB, w.fc_h_a_b, P.ha, AC_EMB, ACT_RELU);          // fc_h_a
+    L.fwd(g, P.ha, AC_EMB, w.fc_z_a_w, AC_EMB, P.atoms, w.fc_z_a_b, P.adv, AC_MAXATOMS, ACT_NONE);   // fc_z_a
+}
+
+int irbpp_dqn_log_prob(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                       int32_t selected_action, const float* shape_feature, const float* map_feature,
+                       const int64_t* actions, int32_t atoms, float* log_p, void* scratch, int64_t scratch_bytes,
+                       void* stream) {
+    GradParams P;
+    int rc = grad_params(P, weights, obs, obs_stride, B, selected_action, shape_feature, map_feature, actions, atoms,
+                         scratch, scratch_bytes);
+    if (rc) return rc;
+    if (!log_p) return fail(nullptr, IRBPP_EINVAL, "null log_p");
+    P.log_p = log_p;
+    const int dev = device_of(obs);
+    DeviceGuard guard(dev);
+    GradLauncher L{P, (cudaStream_t)stream, grad_grid_cap(dev)};
+    grad_forward(P, L);
+    irbpp_grad_logp_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    return launch_status();
+}
+
+int irbpp_dqn_log_prob_backward(const irbpp_dqn_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                                int32_t selected_action, const float* shape_feature, const float* map_feature,
+                                const int64_t* actions, int32_t atoms, const float* grad_log_p,
+                                const irbpp_dqn_grads* grads, float* d_shape_feature, float* d_map_feature,
+                                void* scratch, int64_t scratch_bytes, void* stream) {
+    GradParams P;
+    int rc = grad_params(P, weights, obs, obs_stride, B, selected_action, shape_feature, map_feature, actions, atoms,
+                         scratch, scratch_bytes);
+    if (rc) return rc;
+    if (!grad_log_p || !grads || !d_shape_feature || !d_map_feature) return fail(nullptr, IRBPP_EINVAL, "null backward argument");
+    const irbpp_dqn_grads& d = *grads;
+    float* outs[] = {d.cand1_w, d.cand1_b, d.cand2_w, d.cand2_b, d.proj1_w, d.proj1_b, d.proj2_w, d.proj2_b, d.fc_h_v_w,
+                     d.fc_h_v_b, d.fc_z_v_w, d.fc_z_v_b, d.fc_h_a_w, d.fc_h_a_b, d.fc_z_a_w, d.fc_z_a_b};
+    for (float* p : outs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null gradient output");
+    P.grad_log_p = grad_log_p;
+    const ActorWeights& w = P.w;
+    const int dev = device_of(obs);
+    DeviceGuard guard(dev);
+    GradLauncher L{P, (cudaStream_t)stream, grad_grid_cap(dev)};
+    grad_forward(P, L);
+    irbpp_grad_head_backward_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    // Each in-place DGRAD below overwrites an activation after the last GEMM that reads it.
+    GemmArgs g = L.base();
+    L.all(g);
+    L.wgrad(g, P.dadv, AC_MAXATOMS, atoms, P.ha, AC_EMB, AC_EMB, d.fc_z_a_w, AC_EMB, d.fc_z_a_b);            // fc_z_a
+    L.dgrad(g, P.dadv, AC_MAXATOMS, atoms, w.fc_z_a_w, AC_EMB, AC_EMB, P.ha, AC_EMB, ACT_RELU);             // ha <- d pre fc_h_a
+    L.wgrad(g, P.ha, AC_EMB, AC_EMB, P.emb, AC_EMB, AC_EMB, d.fc_h_a_w, AC_EMB, d.fc_h_a_b);                // fc_h_a
+    L.valid(g);
+    L.dgrad(g, P.ha, AC_EMB, AC_EMB, w.fc_h_a_w, AC_EMB, AC_EMB, P.emb, AC_EMB, ACT_NONE, P.dg, AC_EMB);    // emb <- d emb
+    L.wgrad(g, P.emb, AC_EMB, AC_EMB, P.p0, AC_PROJ, AC_PROJ, d.proj2_w, AC_PROJ, d.proj2_b);              // project_layer.2
+    L.dgrad(g, P.emb, AC_EMB, AC_EMB, w.proj2_w, AC_PROJ, AC_PROJ, P.p0, AC_PROJ, ACT_LEAKY);              // p0 <- d pre0
+    L.wgrad(g, P.p0, AC_PROJ, AC_PROJ, P.ec, AC_EMB, AC_EMB, d.proj1_w + 384, 512, nullptr);               // project_layer.0, rows
+    irbpp_grad_rowsum_kernel<<<B, AC_PROJ, 0, L.s>>>(P);                                                   // S_b
+    L.dgrad(g, P.p0, AC_PROJ, AC_PROJ, w.proj1_w + 384, 512, AC_EMB, P.ec, AC_EMB, ACT_NONE);              // ec <- d ec
+    L.wgrad(g, P.ec, AC_EMB, AC_EMB, P.h1, 32, 32, d.cand2_w, 32, d.cand2_b);                              // init_candidate_embed.2
+    L.dgrad(g, P.ec, AC_EMB, AC_EMB, w.cand2_w, 32, 32, P.h1, 32, ACT_LEAKY);                              // h1 <- d pre h1
+    L.wgrad(g, P.h1, 32, 32, P.cand, 4, 4, d.cand1_w, 4, d.cand1_b);                                       // init_candidate_embed.0
+    L.per_transition(g);
+    L.wgrad(g, P.S, AC_PROJ, AC_PROJ, P.xcat, 384, 384, d.proj1_w, 512, d.proj1_b);                        // project_layer.0, [sf; mf]
+    L.dgrad(g, P.S, AC_PROJ, AC_PROJ, w.proj1_w, 512, AC_EMB, d_shape_feature, AC_EMB, ACT_NONE);
+    L.dgrad(g, P.S, AC_PROJ, AC_PROJ, w.proj1_w + AC_EMB, 512, 256, d_map_feature, 256, ACT_NONE);
+    L.wgrad(g, P.dq, AC_MAXATOMS, atoms, P.hv, AC_EMB, AC_EMB, d.fc_z_v_w, AC_EMB, d.fc_z_v_b);            // fc_z_v
+    L.wgrad(g, P.dhv, AC_EMB, AC_EMB, P.gv, AC_EMB, AC_EMB, d.fc_h_v_w, AC_EMB, d.fc_h_v_b);               // fc_h_v
+    return launch_status();
 }
 
 int irbpp_debug_phase_cycles(irbpp_handle h, int32_t enable, uint64_t* out8) {

@@ -17,7 +17,8 @@ iteration rate.  This module keeps the loop's shape and removes the per-environm
 * ``PrioritizedReplayBank`` -- the reference's replay itself (``memory.py``: float32 sum tree, n-step returns,
   importance weights, stratified draws) for N memories on the device (``csrc/irbpp_replay.cuh``).
 * ``device_learn``         -- ``Agent.learn`` (``agent.py:68-125``) with its two no-grad passes on the device
-  (``DeviceActor.act`` / ``.target``); the gradient pass, the backward pass and the optimiser stay in torch.
+  (``DeviceActor.act`` / ``.target``) and, at the location level with ``gradient="device"``, the candidate-row
+  network of the gradient pass and its backward (``DeviceActor.log_prob``); the optimiser stays in torch.
 
 ``ReplayBank`` samples uniformly; it exists so that the actor loop can be run end to end at N = 4096 and timed
 (``tools/actor_loop.py``).
@@ -300,7 +301,7 @@ class PrioritizedReplayBank(object):
                 self.priority_exponent, self._flags.data_ptr(), self._stream()))
 
 
-def device_learn(agent, bank, online_actor, target_actor):
+def device_learn(agent, bank, online_actor, target_actor, gradient="torch"):
     """``agent.learn(mem)`` (``agent.py:68-125``) on a ``PrioritizedReplayBank``, for either network level (the level
     follows from the actors): ``online_actor`` wraps ``agent.online_net`` and ``target_actor`` wraps
     ``agent.target_net`` (both ``DeviceActor`` or both ``DeviceOrderActor``, read live).  Returns the loss ``[B]`` on
@@ -315,15 +316,29 @@ def device_learn(agent, bank, online_actor, target_actor):
        agent.py:117-121;
     7. ``bank.update_priorities`` with the loss (agent.py:123-124).
 
+    ``gradient="device"`` (location level only) replaces step 2 with ``online_actor.log_prob(states, actions)``: the
+    candidate-row network and its backward pass run as kernels (``irbpp_dqn_log_prob``), while the encoders, the
+    NoisyLinear rebuild, the loss, ``clip_grad_norm_`` and Adam stay in torch.  ``gradient="torch"`` runs the module
+    itself; it is the only path at the order level and the reference the device path is tested against.
+
     One difference from the reference: its three forward passes each draw point indices with ``np.random``
-    (model.py:331, 367); here only the gradient pass does, and the two device passes draw from the counter-based
-    generator of their actors' ``DeviceShapeClouds`` / ``OrderShapeClouds``, one index set per net."""
+    (model.py:331, 367); here the device passes draw from the counter-based generator of their actors'
+    ``DeviceShapeClouds`` / ``OrderShapeClouds``, one index set per pass (with ``gradient="torch"`` the gradient pass
+    draws as the module does)."""
     import torch
     from torch.nn.utils import clip_grad_norm_
+    if gradient not in ("torch", "device"):
+        raise ValueError("gradient must be 'torch' or 'device', got %r" % (gradient,))
+    if gradient == "device" and not callable(getattr(online_actor, "log_prob", None)):
+        raise ValueError("gradient='device' supports the location level (DeviceActor.log_prob); %s has no log_prob"
+                         % type(online_actor).__name__)
     idxs, states, actions, returns, next_states, nonterminals, weights, mem_ids = bank.sample(agent.batch_size)
     B = states.shape[0]
-    log_ps = agent.online_net(states, log=True)
-    log_ps_a = log_ps[torch.arange(B, device=log_ps.device), actions]
+    if gradient == "device":
+        log_ps_a = online_actor.log_prob(states, actions)
+    else:
+        log_ps = agent.online_net(states, log=True)
+        log_ps_a = log_ps[torch.arange(B, device=log_ps.device), actions]
     with torch.no_grad():
         next_actions = online_actor.act(next_states)
         agent.target_net.reset_noise()

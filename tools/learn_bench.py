@@ -11,7 +11,9 @@ forward and torch expressions), cudnn off, except for where the clouds come from
 ``shapeArray[ids]`` on the host in each of its three forward passes, which is not timed here; ``DeviceShapeClouds``
 gathers the same clouds on the device instead.  The device arm is ``device_learn``: the same gradient pass, the online
 argmax through ``DeviceActor.act`` / ``DeviceOrderActor.act`` and the target through ``.target``.  Both arms share the
-bank, start from the same weights and step their own copies.
+bank, start from the same weights and step their own copies.  At the location level a third arm,
+``device_grad``, is ``device_learn(..., gradient="device")``: the device arm with the gradient pass through
+``DeviceActor.log_prob`` (the candidate-row network and its backward as kernels).
 
 Prints one JSON line per workload: ms per call and per part (sample, gradient pass, target = online argmax + target
 pass + projection, step = loss + backward + clip + Adam, priority update) from CUDA events, medians and minima over
@@ -68,10 +70,10 @@ def filled_bank(lib, n, steps, seed, level, dev):
 class Arm(object):
     """One learner: online / target port modules, Adam, and (device arm) the two device actors."""
 
-    def __init__(self, online, target, clouds, support, device_arm, level):
+    def __init__(self, online, target, clouds, support, device_arm, level, device_grad=False):
         self.online, self.target, self.clouds, self.support, self.level = online, target, clouds, support, level
         self.opt = torch.optim.Adam(online.parameters(), lr=LR, eps=ADAM_EPS)
-        self.device_arm = device_arm
+        self.device_arm, self.device_grad = device_arm, device_grad
         if device_arm:
             A = DeviceOrderActor if level == "order" else DeviceActor
             self.on_actor, self.tg_actor = A(online, clouds, support), A(target, clouds, support)
@@ -90,8 +92,11 @@ class Arm(object):
         idxs, states, actions, returns, next_states, nonterminals, weights, mem_ids = bank.sample(batch)
         B = states.shape[0]
         ev[1].record()
-        log_ps = self.online(states, log=True)
-        log_ps_a = log_ps[torch.arange(B, device=states.device), actions]
+        if self.device_grad:
+            log_ps_a = self.on_actor.log_prob(states, actions)
+        else:
+            log_ps = self.online(states, log=True)
+            log_ps_a = log_ps[torch.arange(B, device=states.device), actions]
         ev[2].record()
         gn = GAMMA ** N_STEP
         with torch.no_grad():
@@ -133,6 +138,8 @@ def run(name, level, lib, a, dev):
     support = torch.linspace(V_MIN, V_MAX, ATOMS, device=dev)
     arms = {"torch": Arm(online, target, clouds, support, False, level),
             "device": Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level)}
+    if level == "location":
+        arms["device_grad"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
     times = {n: [] for n in arms}
     for i in range(a.warmup + a.reps):
@@ -148,6 +155,8 @@ def run(name, level, lib, a, dev):
         out[n] = {"ms_median": float(np.median(tot)), "ms_min": float(tot.min()),
                   "parts_ms_median": {p: float(np.median(ts[:, j])) for j, p in enumerate(PARTS)}}
     out["a_star_agreement"] = float(np.mean(arms["device"].agree))
+    for n, ts in times.items():
+        out[n]["ms_min_parts"] = {p: float(ts_p) for p, ts_p in zip(PARTS, np.array(ts).min(0))}
     out["grad_pass_share_of_device_learn"] = out["device"]["parts_ms_median"]["grad_pass"] / out["device"]["ms_median"]
     out["card"] = card()
     print(json.dumps(out))
