@@ -463,6 +463,41 @@ int irbpp_dqn_log_prob_backward(const irbpp_dqn_weights* weights, const float* o
                                 const irbpp_dqn_grads* grads, float* d_shape_feature, float* d_map_feature,
                                 void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---- the height encoder and its backward pass (csrc/irbpp_height_encoder.cuh) ----------------------------------------
+ * DQNBPP's heightEncoder (model.py:258-264, the same module at both network levels): conv 1->16 k4 s2 p1, conv 16->32
+ * k4 s2 p1, conv 32->4 k3 s1 p1, each followed by LeakyReLU, 256 features flattened in (C, H, W) order; the
+ * convolutions irbpp_dqn_act and irbpp_dqn_order_act run.  Handle-free and float32, no atomics: two calls on the same
+ * inputs give bit-identical results.  Sample b's 32 x 32 heightmap is the 1024 contiguous floats at hm + b * hm_stride
+ * (hm_stride >= 1024), so the heightmap columns of observation rows are read in place.  negative_slope must be finite
+ * and >= 0.  No gradient is taken for the heightmap. */
+typedef struct {
+    const float* conv1_w; const float* conv1_b;     /* heightEncoder.conv1 [16, 1, 4, 4], [16] */
+    const float* conv2_w; const float* conv2_b;     /* heightEncoder.conv2 [32, 16, 4, 4], [32] */
+    const float* conv3_w; const float* conv3_b;     /* heightEncoder.conv3 [4, 32, 3, 3], [4] */
+    float negative_slope;                           /* of the three LeakyReLU (nn.LeakyReLU default 0.01) */
+} irbpp_height_encoder_weights;
+
+/* Gradients of the six tensors, float32 device outputs in the layouts of irbpp_height_encoder_weights. */
+typedef struct {
+    float* conv1_w; float* conv1_b;
+    float* conv2_w; float* conv2_b;
+    float* conv3_w; float* conv3_b;
+} irbpp_height_encoder_grads;
+
+/* Bytes of the scratch irbpp_height_encoder_backward needs for B samples (-1 for bad sizes). */
+int64_t irbpp_height_encoder_scratch_bytes(int32_t B);
+
+/* Writes map_feature float32 [B, 256]. */
+int irbpp_height_encoder_forward(const irbpp_height_encoder_weights* weights, const float* hm, int64_t hm_stride,
+                                 int32_t B, float* map_feature, void* stream);
+
+/* Given grad_map_feature float32 [B, 256] = dL/dmap_feature, writes dL/d(tensor) for every tensor of grads, summed over
+ * the B samples (overwritten, not accumulated).  The forward pass is recomputed inside the call.  scratch:
+ * irbpp_height_encoder_scratch_bytes(B) bytes, 256-byte aligned. */
+int irbpp_height_encoder_backward(const irbpp_height_encoder_weights* weights, const float* hm, int64_t hm_stride,
+                                  int32_t B, const float* grad_map_feature, const irbpp_height_encoder_grads* grads,
+                                  void* scratch, int64_t scratch_bytes, void* stream);
+
 /* Profiling aid: when enabled, thread 0 of every CTA adds the SM cycles it spent in each kernel phase
  * (0 scan kernel: load + apply action, 1 scan kernel: observation heightmap + scan + level bitmaps,
  * 2 candidates kernel: contour tasks, 3 candidates kernel: select / pad) to counters 0-3; counters 4-7 count

@@ -68,6 +68,17 @@ class IrbppDqnGrads(ctypes.Structure):
                                          "fc_z_a_w", "fc_z_a_b")]
 
 
+class IrbppHeightEncoderWeights(ctypes.Structure):
+    """``irbpp_height_encoder_weights``: device pointers of the height encoder's six tensors, then the LeakyReLU slope."""
+    _fields_ = [(n, c_void_p) for n in ("conv1_w", "conv1_b", "conv2_w", "conv2_b", "conv3_w", "conv3_b")] + \
+        [("negative_slope", ctypes.c_float)]
+
+
+class IrbppHeightEncoderGrads(ctypes.Structure):
+    """``irbpp_height_encoder_grads``: device pointers of the gradients of the height encoder's six tensors."""
+    _fields_ = [(n, c_void_p) for n in ("conv1_w", "conv1_b", "conv2_w", "conv2_b", "conv3_w", "conv3_b")]
+
+
 # symbol -> (restype, argtypes); every symbol of include/irbpp.h appears here (checked by the tests)
 SIGNATURES = {
     "irbpp_abi_version": (c_i32, []),
@@ -121,6 +132,11 @@ SIGNATURES = {
     "irbpp_dqn_log_prob_backward": (c_i32, [ctypes.POINTER(IrbppDqnWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p,
                                             c_void_p, c_void_p, c_i32, c_void_p, ctypes.POINTER(IrbppDqnGrads), c_void_p,
                                             c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_height_encoder_scratch_bytes": (c_i64, [c_i32]),
+    "irbpp_height_encoder_forward": (c_i32, [ctypes.POINTER(IrbppHeightEncoderWeights), c_void_p, c_i64, c_i32, c_void_p,
+                                             c_void_p]),
+    "irbpp_height_encoder_backward": (c_i32, [ctypes.POINTER(IrbppHeightEncoderWeights), c_void_p, c_i64, c_i32, c_void_p,
+                                              ctypes.POINTER(IrbppHeightEncoderGrads), c_void_p, c_i64, c_void_p]),
     "irbpp_replay_init": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p]),
     "irbpp_replay_append": (c_i32, [ctypes.POINTER(IrbppReplayMemory), c_void_p, c_i64, c_void_p, c_void_p, c_void_p,
                                     c_void_p, ctypes.c_float, c_void_p]),

@@ -25,6 +25,7 @@
 #include "irbpp_actor.cuh"
 #include "irbpp_order_actor.cuh"
 #include "irbpp_grad.cuh"
+#include "irbpp_height_encoder.cuh"
 
 using namespace irbpp;
 
@@ -1381,6 +1382,75 @@ int irbpp_dqn_log_prob_backward(const irbpp_dqn_weights* weights, const float* o
     L.dgrad(g, P.S, AC_PROJ, AC_PROJ, w.proj1_w + AC_EMB, 512, 256, d_map_feature, 256, ACT_NONE);
     L.wgrad(g, P.dq, AC_MAXATOMS, atoms, P.hv, AC_EMB, AC_EMB, d.fc_z_v_w, AC_EMB, d.fc_z_v_b);            // fc_z_v
     L.wgrad(g, P.dhv, AC_EMB, AC_EMB, P.gv, AC_EMB, AC_EMB, d.fc_h_v_w, AC_EMB, d.fc_h_v_b);               // fc_h_v
+    return launch_status();
+}
+
+// ---- the height encoder and its backward pass (csrc/irbpp_height_encoder.cuh) -----------------------------------------
+int64_t irbpp_height_encoder_scratch_bytes(int32_t B) {
+    if (B <= 0) return -1;
+    return height_encoder_scratch_bytes(B);
+}
+
+// the argument checks both entry points share, and the parameter block
+static int height_encoder_params(HeightEncoderParams& P, const irbpp_height_encoder_weights* weights, const float* hm,
+                                 int64_t hm_stride, int32_t B) {
+    if (!weights || !hm) return fail(nullptr, IRBPP_EINVAL, "null height-encoder argument");
+    if (B <= 0) return fail(nullptr, IRBPP_EINVAL, "need B >= 1 samples (B %d)", B);
+    if (hm_stride < AC_HM * AC_HM) return fail(nullptr, IRBPP_EINVAL, "heightmap stride %lld < 1024", (long long)hm_stride);
+    const irbpp_height_encoder_weights& w = *weights;
+    const float* ptrs[] = {w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b};
+    for (const float* p : ptrs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null weight pointer");
+    if (!(w.negative_slope >= 0.0f) || !std::isfinite(w.negative_slope))
+        return fail(nullptr, IRBPP_EINVAL, "negative_slope %g is not a finite value >= 0", (double)w.negative_slope);
+    memset(&P, 0, sizeof(P));
+    P.w = HeightEncoderWeights{w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.negative_slope};
+    P.hm = hm; P.hm_stride = hm_stride; P.B = B;
+    return IRBPP_OK;
+}
+
+int irbpp_height_encoder_forward(const irbpp_height_encoder_weights* weights, const float* hm, int64_t hm_stride,
+                                 int32_t B, float* map_feature, void* stream) {
+    HeightEncoderParams P;
+    int rc = height_encoder_params(P, weights, hm, hm_stride, B);
+    if (rc) return rc;
+    if (!map_feature) return fail(nullptr, IRBPP_EINVAL, "null map_feature");
+    P.map = map_feature;
+    DeviceGuard guard(device_of(hm));
+    irbpp_height_encoder_kernel<<<B, AC_THREADS, 0, (cudaStream_t)stream>>>(P);
+    return launch_status();
+}
+
+int irbpp_height_encoder_backward(const irbpp_height_encoder_weights* weights, const float* hm, int64_t hm_stride,
+                                  int32_t B, const float* grad_map_feature, const irbpp_height_encoder_grads* grads,
+                                  void* scratch, int64_t scratch_bytes, void* stream) {
+    HeightEncoderParams P;
+    int rc = height_encoder_params(P, weights, hm, hm_stride, B);
+    if (rc) return rc;
+    if (!grad_map_feature || !grads || !scratch) return fail(nullptr, IRBPP_EINVAL, "null backward argument");
+    const irbpp_height_encoder_grads& d = *grads;
+    float* outs[] = {d.conv1_w, d.conv1_b, d.conv2_w, d.conv2_b, d.conv3_w, d.conv3_b};
+    for (float* p : outs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null gradient output");
+    if (scratch_bytes < height_encoder_scratch_bytes(B))
+        return fail(nullptr, IRBPP_EINVAL, "scratch of %lld bytes < %lld", (long long)scratch_bytes, (long long)height_encoder_scratch_bytes(B));
+    if (reinterpret_cast<uintptr_t>(scratch) & 255) return fail(nullptr, IRBPP_EINVAL, "scratch not 256-byte aligned");
+    P.d_map = grad_map_feature;
+    P.part = static_cast<float*>(scratch);
+    const int dev = device_of(hm);
+    DeviceGuard guard(dev);
+    cudaStream_t s = (cudaStream_t)stream;
+    irbpp_height_encoder_backward_kernel<<<B, AC_THREADS, 0, s>>>(P);
+    const HeightEncoderGrads G{d.conv1_w, d.conv1_b, d.conv2_w, d.conv2_b, d.conv3_w, d.conv3_b};
+    int64_t rows = B, stride = HE_GRADS;
+    for (;;) {                                   // groups of HE_GROUP samples, in place, until one row is left
+        const int64_t groups = (rows + HE_GROUP - 1) / HE_GROUP;
+        const int64_t blocks = std::min<int64_t>((groups * HE_GRADS + AC_THREADS - 1) / AC_THREADS, gather_grid_cap(dev));
+        irbpp_height_encoder_reduce_kernel<<<(int)blocks, AC_THREADS, 0, s>>>(P.part, stride, (int32_t)rows, G);
+        if (groups == 1) break;
+        rows = groups;
+        stride *= HE_GROUP;
+    }
     return launch_status();
 }
 

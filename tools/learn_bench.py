@@ -13,13 +13,20 @@ gathers the same clouds on the device instead.  The device arm is ``device_learn
 argmax through ``DeviceActor.act`` / ``DeviceOrderActor.act`` and the target through ``.target``.  Both arms share the
 bank, start from the same weights and step their own copies.  At the location level a third arm,
 ``device_grad``, is ``device_learn(..., gradient="device")``: the device arm with the gradient pass through
-``DeviceActor.log_prob`` (the candidate-row network and its backward as kernels).
+``DeviceActor.log_prob`` (the candidate-row network and its backward as kernels).  The ``*_enc`` arms repeat
+``device_grad`` (location) and ``device`` (order) with ``DeviceHeightEncoder`` swapped into the online net, so the
+height encoder and its backward pass run as kernels too.
 
 Prints one JSON line per workload: ms per call and per part (sample, gradient pass, target = online argmax + target
 pass + projection, step = loss + backward + clip + Adam, priority update) from CUDA events, medians and minima over
 ``--reps`` calls after ``--warmup``; the fraction of samples whose a* agrees between the two arms (the torch argmax
 evaluated on the device arm's batches with the device arm's point indices); the card's name and power limit read in
-the same run."""
+the same run.
+
+Before those, one JSON line per batch size for the height encoder alone (``bench: height_encoder``): the forward pass at
+B = 4096 (an act over 4096 bins) and forward + backward at B = 64 and 512, ``DeviceHeightEncoder`` against torch
+float32 (TF32 off) with cudnn off, as the reference trains, and with cudnn on; median and minimum ms per call from
+CUDA events.  ``--encoder-only`` prints only these lines."""
 import argparse
 import copy
 import json
@@ -32,9 +39,11 @@ import torch
 
 from irbpp_b200 import shapes
 from irbpp_b200.actor import DeviceActor, DeviceOrderActor
+from irbpp_b200.height_encoder import DeviceHeightEncoder
 from irbpp_b200.learner_glue import PrioritizedReplayBank, get_mask_from_state
 from irbpp_b200.pointnet import DeviceShapeClouds
 from irbpp_b200.vec_env import GpuVecEnv
+from oracle.dqn_port import DQNPort
 from oracle.learn_port import ReferenceDQN, ReferenceOrderDQN, distribution, torch_projection
 from tools.act_bench import card
 
@@ -70,7 +79,9 @@ def filled_bank(lib, n, steps, seed, level, dev):
 class Arm(object):
     """One learner: online / target port modules, Adam, and (device arm) the two device actors."""
 
-    def __init__(self, online, target, clouds, support, device_arm, level, device_grad=False):
+    def __init__(self, online, target, clouds, support, device_arm, level, device_grad=False, device_encoder=False):
+        if device_encoder:
+            online.heightEncoder = DeviceHeightEncoder(online.heightEncoder)
         self.online, self.target, self.clouds, self.support, self.level = online, target, clouds, support, level
         self.opt = torch.optim.Adam(online.parameters(), lr=LR, eps=ADAM_EPS)
         self.device_arm, self.device_grad = device_arm, device_grad
@@ -140,6 +151,11 @@ def run(name, level, lib, a, dev):
             "device": Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level)}
     if level == "location":
         arms["device_grad"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True)
+        arms["device_grad_enc"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True,
+                                      True)
+    else:
+        arms["device_enc"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, False,
+                                 True)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
     times = {n: [] for n in arms}
     for i in range(a.warmup + a.reps):
@@ -162,15 +178,63 @@ def run(name, level, lib, a, dev):
     print(json.dumps(out))
 
 
+def time_calls(fn, reps, warmup):
+    """median and minimum ms of ``fn()`` over ``reps`` calls after ``warmup``, CUDA events around each call"""
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    ts = []
+    for i in range(warmup + reps):
+        ev[0].record()
+        fn()
+        ev[1].record()
+        torch.cuda.synchronize()
+        if i >= warmup:
+            ts.append(ev[0].elapsed_time(ev[1]))
+    return {"ms_median": float(np.median(ts)), "ms_min": float(np.min(ts))}
+
+
+def encoder_bench(a, dev):
+    """The height encoder alone: heightmaps read in place from observation rows of the location level's width."""
+    torch.manual_seed(0)
+    seq = DQNPort(selected_action=SEL, atoms=ATOMS).heightEncoder.to(dev)
+    arms = {"device": DeviceHeightEncoder(copy.deepcopy(seq)), "torch": seq}
+    for B, backward in ((4096, False), (64, True), (512, True)):
+        rows = torch.rand((B, SEL * 5 + 9 + 1024), device=dev) * 0.3
+        hm = rows[:, SEL * 5 + 9:].reshape(B, 1, 32, 32)
+        g = torch.randn((B, 4, 8, 8), device=dev)
+        out = {"bench": "height_encoder", "batch": B, "pass": "forward+backward" if backward else "forward",
+               "reps": a.reps}
+
+        def call(enc):
+            if backward:
+                for p in enc.parameters():
+                    p.grad = None
+                enc(hm).backward(g)
+            else:
+                with torch.no_grad():
+                    enc(hm)
+        for name, enc, cudnn in (("device", arms["device"], False), ("torch_cudnn_off", arms["torch"], False),
+                                 ("torch_cudnn_on", arms["torch"], True)):
+            with torch.backends.cudnn.flags(enabled=cudnn, allow_tf32=False):
+                out[name] = time_calls(lambda: call(enc), a.reps, a.warmup)
+        for name in ("torch_cudnn_off", "torch_cudnn_on"):
+            out["speedup_vs_" + name] = out[name]["ms_median"] / out["device"]["ms_median"]
+        out["card"] = card()
+        print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--bins", type=int, default=4096)
     ap.add_argument("--reps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--encoder-only", action="store_true")
     a = ap.parse_args()
     torch.backends.cudnn.enabled = False
     dev = torch.device("cuda:0")
+    encoder_bench(a, dev)
+    if a.encoder_only:
+        return
     run("blockout", "location", shapes.make_blockout_library(32, seed=1), a, dev)
     run("general", "location", shapes.make_irregular_library(16, seed=2, num_rotations=8), a, dev)
     run("blockout_buffered", "order", shapes.make_blockout_library(32, seed=1), a, dev)
