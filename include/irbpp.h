@@ -463,6 +463,57 @@ int irbpp_dqn_log_prob_backward(const irbpp_dqn_weights* weights, const float* o
                                 const irbpp_dqn_grads* grads, float* d_shape_feature, float* d_map_feature,
                                 void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---- the gradient pass of Agent.learn at the order level (csrc/irbpp_order_grad.cuh) ---------------------------------
+ * The order network of DQNBPP (args.level == 'order', bufferSize k > 1) from its inputs to log p(s, a_t, .)
+ * (agent.py:85-86 with model.py:355-383, 386-404), and its backward pass: gat_project_layer, the single-head
+ * graph-attention layer over the k slots of a bin (nothing masked), its feed-forward block, both residuals, the slot
+ * mean and the dueling heads.  The caller computes, with autograd, shape_features [S, 128] (shapeEncoder on every
+ * library shape, max over the points, one index set shared by the batch) and map_feature [B, 256] (heightEncoder), and
+ * the NoisyLinear effective weights; the kernels take them as inputs and return their gradients.  Handle-free, like
+ * irbpp_dqn_order_act, with its weight conventions; the heightEncoder fields of irbpp_dqn_order_weights are not read and
+ * may be NULL.  Supported: hidden_size 128, 2 <= k <= 32, 1 <= atoms <= 32, S >= 1, B * k * 384 < 2^31.  An item id
+ * is read as (int) obs[b, j] and clamped to [0, S), an action outside [0, k) is clamped into it (the reference raises
+ * IndexError for both).  Float32 throughout, no atomics: two calls on the same inputs give bit-identical results. */
+
+/* Gradients of the effective tensors of irbpp_dqn_order_weights after the six convolutions, one float32 device output
+ * per field, each in that field's layout. */
+typedef struct {
+    float* gat1_w; float* gat1_b;       /* gat_project_layer.0 [256, 384], [256] */
+    float* gat2_w; float* gat2_b;       /* gat_project_layer.2 [128, 256], [128] */
+    float* wq; float* wk; float* wv;    /* W_query, W_key, W_val [128, 128] */
+    float* wo_w; float* wo_b;           /* W_out [128, 128], [128] */
+    float* ff1_w; float* ff1_b;         /* feed-forward Linear 0 [128, 128], [128] */
+    float* ff2_w; float* ff2_b;         /* feed-forward Linear 2 [128, 128], [128] */
+    float* fc_h_v_w; float* fc_h_v_b;   /* fc_h_v [128, 128], [128] */
+    float* fc_z_v_w; float* fc_z_v_b;   /* fc_z_v [atoms, 128], [atoms] */
+    float* fc_h_a_w; float* fc_h_a_b;   /* fc_h_a [128, 128], [128] */
+    float* fc_z_a_w; float* fc_z_a_b;   /* fc_z_a [atoms, 128], [atoms] */
+} irbpp_dqn_order_grads;
+
+/* Bytes of the scratch irbpp_dqn_order_log_prob and irbpp_dqn_order_log_prob_backward need for B transitions of k
+ * slots and S library shapes (-1 for bad sizes). */
+int64_t irbpp_dqn_order_log_prob_scratch_bytes(int32_t B, int32_t k, int32_t S);
+
+/* obs float32 [B] rows of obs_stride >= k + 1024 (the sampled order states: k item ids as floats, the 32 x 32
+ * heightmap), shape_features float32 [S, 128], map_feature float32 [B, 256], actions int64 [B] (a_t).  Writes log_p
+ * float32 [B, atoms] = log_softmax(q(s, a_t)) computed as q - max - log sum exp(q - max).  scratch:
+ * irbpp_dqn_order_log_prob_scratch_bytes bytes, 256-byte aligned. */
+int irbpp_dqn_order_log_prob(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                             int32_t k, const float* shape_features, int32_t S, const float* map_feature,
+                             const int64_t* actions, int32_t atoms, float* log_p, void* scratch, int64_t scratch_bytes,
+                             void* stream);
+
+/* The backward pass of irbpp_dqn_order_log_prob on the same inputs: given grad_log_p float32 [B, atoms] = dL/dlog_p,
+ * writes dL/d(tensor) for every tensor of grads (overwritten, not accumulated), d_shape_features float32 [S, 128] (zero
+ * for a shape no slot holds) and d_map_feature float32 [B, 256].  The forward pass is recomputed inside the call; the
+ * scratch is the forward's size. */
+int irbpp_dqn_order_log_prob_backward(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride,
+                                      int32_t B, int32_t k, const float* shape_features, int32_t S,
+                                      const float* map_feature, const int64_t* actions, int32_t atoms,
+                                      const float* grad_log_p, const irbpp_dqn_order_grads* grads,
+                                      float* d_shape_features, float* d_map_feature, void* scratch,
+                                      int64_t scratch_bytes, void* stream);
+
 /* ---- the height encoder and its backward pass (csrc/irbpp_height_encoder.cuh) ----------------------------------------
  * DQNBPP's heightEncoder (model.py:258-264, the same module at both network levels): conv 1->16 k4 s2 p1, conv 16->32
  * k4 s2 p1, conv 32->4 k3 s1 p1, each followed by LeakyReLU, 256 features flattened in (C, H, W) order; the

@@ -68,6 +68,13 @@ class IrbppDqnGrads(ctypes.Structure):
                                          "fc_z_a_w", "fc_z_a_b")]
 
 
+class IrbppDqnOrderGrads(ctypes.Structure):
+    """``irbpp_dqn_order_grads``: device pointers of the gradients of the order network's tensors after the convolutions."""
+    _fields_ = [(n, c_void_p) for n in ("gat1_w", "gat1_b", "gat2_w", "gat2_b", "wq", "wk", "wv", "wo_w", "wo_b", "ff1_w",
+                                         "ff1_b", "ff2_w", "ff2_b", "fc_h_v_w", "fc_h_v_b", "fc_z_v_w", "fc_z_v_b",
+                                         "fc_h_a_w", "fc_h_a_b", "fc_z_a_w", "fc_z_a_b")]
+
+
 class IrbppHeightEncoderWeights(ctypes.Structure):
     """``irbpp_height_encoder_weights``: device pointers of the height encoder's six tensors, then the LeakyReLU slope."""
     _fields_ = [(n, c_void_p) for n in ("conv1_w", "conv1_b", "conv2_w", "conv2_b", "conv3_w", "conv3_b")] + \
@@ -132,6 +139,13 @@ SIGNATURES = {
     "irbpp_dqn_log_prob_backward": (c_i32, [ctypes.POINTER(IrbppDqnWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p,
                                             c_void_p, c_void_p, c_i32, c_void_p, ctypes.POINTER(IrbppDqnGrads), c_void_p,
                                             c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_dqn_order_log_prob_scratch_bytes": (c_i64, [c_i32, c_i32, c_i32]),
+    "irbpp_dqn_order_log_prob": (c_i32, [ctypes.POINTER(IrbppDqnOrderWeights), c_void_p, c_i64, c_i32, c_i32, c_void_p,
+                                         c_i32, c_void_p, c_void_p, c_i32, c_void_p, c_void_p, c_i64, c_void_p]),
+    "irbpp_dqn_order_log_prob_backward": (c_i32, [ctypes.POINTER(IrbppDqnOrderWeights), c_void_p, c_i64, c_i32, c_i32,
+                                                  c_void_p, c_i32, c_void_p, c_void_p, c_i32, c_void_p,
+                                                  ctypes.POINTER(IrbppDqnOrderGrads), c_void_p, c_void_p, c_void_p, c_i64,
+                                                  c_void_p]),
     "irbpp_height_encoder_scratch_bytes": (c_i64, [c_i32]),
     "irbpp_height_encoder_forward": (c_i32, [ctypes.POINTER(IrbppHeightEncoderWeights), c_void_p, c_i64, c_i32, c_void_p,
                                              c_void_p]),

@@ -514,3 +514,99 @@ class DeviceOrderActor(_NetworkSource):
         _lib.check(self._lib, None, rc)
         self._keep = (ws, enc, shape_features, state, a, r, nt)
         return m, p
+
+    def log_prob(self, states, actions):
+        """``online_net(states, log=True)[arange(B), actions]`` of the order network's ``learn`` (agent.py:85-86,
+        trainer.py:318): float32 ``[B, atoms]``, differentiable with respect to every parameter of the live module the
+        forward pass uses.  torch computes the height encoder, the shape encoder on ``clouds.sample(arange(S))`` (one
+        index set for the batch, as act draws it) and the NoisyLinear effective weights with autograd;
+        ``irbpp_dqn_order_log_prob`` / ``irbpp_dqn_order_log_prob_backward`` run everything per slot and per bin and its
+        backward pass.  ``actions`` (a_t, ``[B]``) are clamped to the k slots and item ids to the library, where the
+        reference raises ``IndexError``.  Double backward is not supported."""
+        torch = self._torch
+        if self.net is None:
+            raise ValueError("log_prob trains the live module; a state-dict actor has no parameters")
+        state, k = self._check_state(states)
+        B = state.shape[0]
+        if not isinstance(actions, torch.Tensor) or actions.device != self.device or actions.numel() != B:
+            raise ValueError("actions must be a tensor of %d values on %s" % (B, self.device))
+        if self.clouds is None:
+            raise ValueError("log_prob samples every library shape's points: the actor needs a DeviceShapeClouds")
+        self._state()                                            # the weights' device
+        net = self.net
+        params = dict(net.named_parameters())
+        params.update(net.named_buffers())
+        eff = {}
+        for m in NOISY:                                          # model.py:224-228, with autograd
+            if net.training:
+                eff[m + ".weight"] = params[m + ".weight_mu"] + params[m + ".weight_sigma"] * params[m + ".weight_epsilon"]
+                eff[m + ".bias"] = params[m + ".bias_mu"] + params[m + ".bias_sigma"] * params[m + ".bias_epsilon"]
+            else:
+                eff[m + ".weight"], eff[m + ".bias"] = params[m + ".weight_mu"], params[m + ".bias_mu"]
+        weights = [(eff[key] if key in eff else params[key]).to(torch.float32).contiguous() for _, key in _ORDER_ROW_FIELDS]
+        hm = state[:, k:k + HM * HM].reshape(B, 1, HM, HM)
+        map_feature = net.heightEncoder(hm).reshape(B, -1)                            # model.py:361-363
+        ids = torch.arange(self.clouds.S, dtype=torch.int32, device=self.device)
+        shape_features = net.shapeEncoder(self.clouds.sample(ids)).max(1)[0]         # model.py:365-372, per shape
+        a = actions.detach().reshape(B).to(torch.int64).contiguous()
+        return _order_log_prob_function().apply(self, state, k, a, shape_features.to(torch.float32).contiguous(),
+                                                map_feature.to(torch.float32).contiguous(), *weights)
+
+
+# the fields of irbpp_dqn_order_weights after the convolutions: the tensors irbpp_dqn_order_log_prob reads and
+# irbpp_dqn_order_grads returns
+_ORDER_ROW_FIELDS = _ORDER_FIELDS[6:]
+_ORDER_LOG_PROB = []
+
+
+def _order_log_prob_function():
+    """The ``torch.autograd.Function`` behind ``DeviceOrderActor.log_prob`` (built once; torch is imported lazily)."""
+    if _ORDER_LOG_PROB:
+        return _ORDER_LOG_PROB[0]
+    import torch
+
+    def weights_struct(ws):
+        ptrs = dict((f, t.data_ptr()) for (f, _), t in zip(_ORDER_ROW_FIELDS, ws))
+        return _lib.IrbppDqnOrderWeights(*([ptrs.get(f, 0) for f, _ in _ORDER_FIELDS] + [ctypes.c_float(0.01)]))
+
+    class OrderLogProb(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, actor, state, k, actions, shape_features, map_feature, *ws):
+            B, S = state.shape[0], shape_features.shape[0]
+            lib = actor._lib
+            w = weights_struct(ws)
+            scratch = actor._scratch_of(int(lib.irbpp_dqn_order_log_prob_scratch_bytes(B, k, S)))
+            log_p = torch.empty((B, actor.atoms), dtype=torch.float32, device=actor.device)
+            rc = lib.irbpp_dqn_order_log_prob(ctypes.byref(w), state.data_ptr(), state.stride(0), B, k,
+                                              shape_features.data_ptr(), S, map_feature.data_ptr(), actions.data_ptr(),
+                                              actor.atoms, log_p.data_ptr(), scratch.data_ptr(), scratch.numel(),
+                                              torch.cuda.current_stream(actor.device).cuda_stream)
+            _lib.check(lib, None, rc)
+            ctx.actor, ctx.state, ctx.k, ctx.actions = actor, state, k, actions
+            ctx.save_for_backward(shape_features, map_feature, *ws)
+            return log_p
+
+        @staticmethod
+        @torch.autograd.function.once_differentiable
+        def backward(ctx, grad):
+            actor, state, k, actions = ctx.actor, ctx.state, ctx.k, ctx.actions
+            shape_features, map_feature = ctx.saved_tensors[:2]
+            ws = ctx.saved_tensors[2:]
+            B, S, lib = state.shape[0], shape_features.shape[0], actor._lib
+            grad = grad.to(torch.float32).contiguous()
+            w = weights_struct(ws)
+            dws = [torch.empty_like(t) for t in ws]
+            g = _lib.IrbppDqnOrderGrads(*[t.data_ptr() for t in dws])
+            d_sf, d_mf = torch.empty_like(shape_features), torch.empty_like(map_feature)
+            scratch = actor._scratch_of(int(lib.irbpp_dqn_order_log_prob_scratch_bytes(B, k, S)))
+            rc = lib.irbpp_dqn_order_log_prob_backward(ctypes.byref(w), state.data_ptr(), state.stride(0), B, k,
+                                                       shape_features.data_ptr(), S, map_feature.data_ptr(),
+                                                       actions.data_ptr(), actor.atoms, grad.data_ptr(), ctypes.byref(g),
+                                                       d_sf.data_ptr(), d_mf.data_ptr(), scratch.data_ptr(),
+                                                       scratch.numel(), torch.cuda.current_stream(actor.device).cuda_stream)
+            _lib.check(lib, None, rc)
+            actor._keep = (grad, ws, state, actions)             # alive until the next call: the launches are asynchronous
+            return (None, None, None, None, d_sf, d_mf) + tuple(dws)
+
+    _ORDER_LOG_PROB.append(OrderLogProb)
+    return OrderLogProb

@@ -26,6 +26,7 @@
 #include "irbpp_order_actor.cuh"
 #include "irbpp_grad.cuh"
 #include "irbpp_height_encoder.cuh"
+#include "irbpp_order_grad.cuh"
 
 using namespace irbpp;
 
@@ -1250,22 +1251,24 @@ static int grad_params(GradParams& P, const irbpp_dqn_weights* weights, const fl
     return IRBPP_OK;
 }
 
-// one GEMM of csrc/irbpp_grad.cuh: rows [row0, row0 + rows_host + *rows_dev), at most rows_max of them
-struct GradLauncher {
-    const GradParams& P;
+// one GEMM of csrc/irbpp_grad.cuh: rows [row0, row0 + rows_host + *rows_dev), at most rows_max of them.  owner, slope
+// and the weight-gradient slices come from the caller's parameter block; dev_rows_max bounds *rows_dev.
+struct GemmLauncher {
     cudaStream_t s;
     int64_t cap;
+    const int32_t* owner;
+    float slope;
+    float* part;
+    int64_t dev_rows_max;
     GemmArgs base() const {
         GemmArgs g;
         memset(&g, 0, sizeof(g));
-        g.owner = P.owner; g.slope = P.w.slope;
+        g.owner = owner; g.slope = slope;
         return g;
     }
-    // all rows (stand-ins and valid rows), the valid rows, the B transitions
-    void all(GemmArgs& g) const { g.row0 = 0; g.rows_host = P.B; g.rows_dev = P.count; }
-    void valid(GemmArgs& g) const { g.row0 = P.B; g.rows_host = 0; g.rows_dev = P.count; }
-    void per_transition(GemmArgs& g) const { g.row0 = 0; g.rows_host = P.B; g.rows_dev = nullptr; }
-    int64_t rows_max(const GemmArgs& g) const { return g.rows_host + (g.rows_dev ? (int64_t)P.B * P.sel : 0); }
+    // the first n rows, a count known on the host
+    void first(GemmArgs& g, int n) const { g.row0 = 0; g.rows_host = n; g.rows_dev = nullptr; }
+    int64_t rows_max(const GemmArgs& g) const { return g.rows_host + (g.rows_dev ? dev_rows_max : 0); }
     int grid(int64_t tiles) const { return (int)std::max<int64_t>(1, std::min<int64_t>(tiles, cap)); }
     // out[r][n] = act(in[r][:] . W[n][:] + bias[n] (+ add[owner r][n]))
     void fwd(GemmArgs g, const float* in, int K, const float* W, int ldw, int N, const float* bias, float* out, int ldo,
@@ -1283,12 +1286,23 @@ struct GradLauncher {
     }
     // dW[n][k] (row stride ldo) = sum_r dy[r][n] x[r][k], db[n] = sum_r dy[r][n] (db may be NULL)
     void wgrad(GemmArgs g, const float* dy, int ldy, int N, const float* x, int ldx, int K, float* dw, int ldo, float* db) const {
-        g.a = dy; g.lda = ldy; g.b = x; g.ldb = ldx; g.c = P.part; g.ldc = K; g.M = N; g.N = K;
+        g.a = dy; g.lda = ldy; g.b = x; g.ldb = ldx; g.c = part; g.ldc = K; g.M = N; g.N = K;
         const int64_t tiles = (int64_t)((N + GR_TILE - 1) / GR_TILE) * ((K + GR_TILE - 1) / GR_TILE) * GR_CHUNKS;
         irbpp_grad_wgrad_kernel<<<grid(tiles), GR_THREADS, 0, s>>>(g);
         irbpp_grad_reduce_kernel<<<grid(((int64_t)N * K + N + GR_THREADS - 1) / GR_THREADS), GR_THREADS, 0, s>>>(
-            P.part, N, K, K, dw, ldo, db);
+            part, N, K, K, dw, ldo, db);
     }
+};
+
+// the location level's row spaces
+struct GradLauncher : GemmLauncher {
+    const GradParams& P;
+    GradLauncher(const GradParams& P_, cudaStream_t s_, int64_t cap_)
+        : GemmLauncher{s_, cap_, P_.owner, P_.w.slope, P_.part, (int64_t)P_.B * P_.sel}, P(P_) {}
+    // all rows (stand-ins and valid rows), the valid rows, the B transitions
+    void all(GemmArgs& g) const { g.row0 = 0; g.rows_host = P.B; g.rows_dev = P.count; }
+    void valid(GemmArgs& g) const { g.row0 = P.B; g.rows_host = 0; g.rows_dev = P.count; }
+    void per_transition(GemmArgs& g) const { first(g, P.B); }
 };
 
 // CTAs per GEMM launch: four per SM on the device.  The tile loop and the fixed row slices make the results independent
@@ -1451,6 +1465,148 @@ int irbpp_height_encoder_backward(const irbpp_height_encoder_weights* weights, c
         rows = groups;
         stride *= HE_GROUP;
     }
+    return launch_status();
+}
+
+// ---- the gradient pass of Agent.learn at the order level (csrc/irbpp_order_grad.cuh) ---------------------------------
+int64_t irbpp_dqn_order_log_prob_scratch_bytes(int32_t B, int32_t k, int32_t S) {
+    if (B <= 0 || k < 2 || k > OA_MAXK || S <= 0 || (int64_t)B * k * 384 >= INT32_MAX) return -1;
+    return order_grad_scratch_bytes(B, k, S);
+}
+
+// the argument checks both entry points share, and the parameter block
+static int order_grad_params(OrderGradParams& P, const irbpp_dqn_order_weights* weights, const float* obs,
+                             int64_t obs_stride, int32_t B, int32_t k, const float* shape_features, int32_t S,
+                             const float* map_feature, const int64_t* actions, int32_t atoms, void* scratch,
+                             int64_t scratch_bytes) {
+    if (!weights || !obs || !shape_features || !map_feature || !actions || !scratch)
+        return fail(nullptr, IRBPP_EINVAL, "null order log-prob argument");
+    if (B <= 0 || S <= 0) return fail(nullptr, IRBPP_EINVAL, "need B >= 1 transitions and S >= 1 shapes (B %d, S %d)", B, S);
+    if (k < 2 || k > OA_MAXK) return fail(nullptr, IRBPP_EINVAL, "buffer size k %d outside [2, %d]", k, OA_MAXK);
+    if ((int64_t)B * k * 384 >= INT32_MAX) return fail(nullptr, IRBPP_EINVAL, "B * k too large (B %d, k %d)", B, k);
+    if (atoms < 1 || atoms > AC_MAXATOMS) return fail(nullptr, IRBPP_EINVAL, "atoms %d outside [1, %d]", atoms, AC_MAXATOMS);
+    if (obs_stride < (int64_t)k + AC_HM * AC_HM)
+        return fail(nullptr, IRBPP_EINVAL, "observation stride %lld < k + 1024", (long long)obs_stride);
+    if (scratch_bytes < order_grad_scratch_bytes(B, k, S))
+        return fail(nullptr, IRBPP_EINVAL, "scratch of %lld bytes < %lld", (long long)scratch_bytes, (long long)order_grad_scratch_bytes(B, k, S));
+    if (reinterpret_cast<uintptr_t>(scratch) & 255) return fail(nullptr, IRBPP_EINVAL, "scratch not 256-byte aligned");
+    const irbpp_dqn_order_weights& w = *weights;
+    const float* ptrs[] = {w.gat1_w, w.gat1_b, w.gat2_w, w.gat2_b, w.wq, w.wk, w.wv, w.wo_w, w.wo_b, w.ff1_w, w.ff1_b,
+                           w.ff2_w, w.ff2_b, w.fc_h_v_w, w.fc_h_v_b, w.fc_z_v_w, w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b,
+                           w.fc_z_a_w, w.fc_z_a_b};
+    for (const float* p : ptrs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null weight pointer");
+    memset(&P, 0, sizeof(P));
+    P.w = OrderWeights{w.conv1_w, w.conv1_b, w.conv2_w, w.conv2_b, w.conv3_w, w.conv3_b, w.gat1_w, w.gat1_b, w.gat2_w,
+                       w.gat2_b, w.wq, w.wk, w.wv, w.wo_w, w.wo_b, w.ff1_w, w.ff1_b, w.ff2_w, w.ff2_b, w.fc_h_v_w,
+                       w.fc_h_v_b, w.fc_z_v_w, w.fc_z_v_b, w.fc_h_a_w, w.fc_h_a_b, w.fc_z_a_w, w.fc_z_a_b, w.negative_slope};
+    P.obs = obs; P.obs_stride = obs_stride; P.B = B; P.k = k; P.S = S; P.atoms = atoms;
+    P.shape_features = shape_features; P.map_feature = map_feature; P.actions = actions;
+    order_grad_scratch_layout(P, scratch);
+    return IRBPP_OK;
+}
+
+static void order_grad_add(float* y, const float* x, int64_t n, const GemmLauncher& L) {
+    irbpp_order_grad_add_kernel<<<L.grid((n + GR_THREADS - 1) / GR_THREADS), GR_THREADS, 0, L.s>>>(y, x, n);
+}
+
+// the forward pass into the scratch; log_p written by the head when P.log_p is set
+static void order_grad_forward(const OrderGradParams& P, const GemmLauncher& L) {
+    const OrderWeights& w = P.w;
+    const int B = P.B, R = P.B * P.k;
+    irbpp_order_grad_prep_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    GemmArgs g = L.base();
+    L.first(g, B);
+    L.fwd(g, P.map_feature, 256, w.gat1_w + AC_EMB, 384, AC_PROJ, w.gat1_b, P.u, AC_PROJ, ACT_NONE);     // u_b
+    L.first(g, R);
+    L.fwd(g, P.xs, AC_EMB, w.gat1_w, 384, AC_PROJ, nullptr, P.p0, AC_PROJ, ACT_LEAKY, P.u, AC_PROJ);      // gat_project_layer.0
+    L.fwd(g, P.p0, AC_PROJ, w.gat2_w, AC_PROJ, AC_EMB, w.gat2_b, P.h, AC_EMB, ACT_NONE);                  // gat_project_layer.2
+    L.fwd(g, P.h, AC_EMB, P.wqkv, AC_EMB, 384, nullptr, P.qkv, 384, ACT_NONE);                            // Q | K | V
+    irbpp_order_grad_attn_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    L.fwd(g, P.heads, AC_EMB, w.wo_w, AC_EMB, AC_EMB, w.wo_b, P.h1, AC_EMB, ACT_NONE);                    // W_out
+    order_grad_add(P.h1, P.h, (int64_t)R * AC_EMB, L);                                                    // h1
+    L.fwd(g, P.h1, AC_EMB, w.ff1_w, AC_EMB, AC_EMB, w.ff1_b, P.f1, AC_EMB, ACT_RELU);                    // FFN
+    L.fwd(g, P.f1, AC_EMB, w.ff2_w, AC_EMB, AC_EMB, w.ff2_b, P.h2, AC_EMB, ACT_NONE);
+    order_grad_add(P.h2, P.h1, (int64_t)R * AC_EMB, L);                                                   // h2
+    L.fwd(g, P.h2, AC_EMB, w.fc_h_a_w, AC_EMB, AC_EMB, w.fc_h_a_b, P.ha, AC_EMB, ACT_RELU);              // fc_h_a
+    L.fwd(g, P.ha, AC_EMB, w.fc_z_a_w, AC_EMB, P.atoms, w.fc_z_a_b, P.adv, AC_MAXATOMS, ACT_NONE);       // fc_z_a
+}
+
+int irbpp_dqn_order_log_prob(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride, int32_t B,
+                             int32_t k, const float* shape_features, int32_t S, const float* map_feature,
+                             const int64_t* actions, int32_t atoms, float* log_p, void* scratch, int64_t scratch_bytes,
+                             void* stream) {
+    OrderGradParams P;
+    int rc = order_grad_params(P, weights, obs, obs_stride, B, k, shape_features, S, map_feature, actions, atoms, scratch,
+                               scratch_bytes);
+    if (rc) return rc;
+    if (!log_p) return fail(nullptr, IRBPP_EINVAL, "null log_p");
+    P.log_p = log_p;
+    const int dev = device_of(obs);
+    DeviceGuard guard(dev);
+    const GemmLauncher L{(cudaStream_t)stream, grad_grid_cap(dev), P.owner, P.w.slope, P.part, 0};
+    order_grad_forward(P, L);
+    irbpp_order_grad_logp_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    return launch_status();
+}
+
+int irbpp_dqn_order_log_prob_backward(const irbpp_dqn_order_weights* weights, const float* obs, int64_t obs_stride,
+                                      int32_t B, int32_t k, const float* shape_features, int32_t S,
+                                      const float* map_feature, const int64_t* actions, int32_t atoms,
+                                      const float* grad_log_p, const irbpp_dqn_order_grads* grads,
+                                      float* d_shape_features, float* d_map_feature, void* scratch,
+                                      int64_t scratch_bytes, void* stream) {
+    OrderGradParams P;
+    int rc = order_grad_params(P, weights, obs, obs_stride, B, k, shape_features, S, map_feature, actions, atoms, scratch,
+                               scratch_bytes);
+    if (rc) return rc;
+    if (!grad_log_p || !grads || !d_shape_features || !d_map_feature)
+        return fail(nullptr, IRBPP_EINVAL, "null backward argument");
+    const irbpp_dqn_order_grads& d = *grads;
+    float* outs[] = {d.gat1_w, d.gat1_b, d.gat2_w, d.gat2_b, d.wq, d.wk, d.wv, d.wo_w, d.wo_b, d.ff1_w, d.ff1_b, d.ff2_w,
+                     d.ff2_b, d.fc_h_v_w, d.fc_h_v_b, d.fc_z_v_w, d.fc_z_v_b, d.fc_h_a_w, d.fc_h_a_b, d.fc_z_a_w, d.fc_z_a_b};
+    for (float* p : outs)
+        if (!p) return fail(nullptr, IRBPP_EINVAL, "null gradient output");
+    P.grad_log_p = grad_log_p;
+    const OrderWeights& w = P.w;
+    const int R = B * k;
+    const int dev = device_of(obs);
+    DeviceGuard guard(dev);
+    const GemmLauncher L{(cudaStream_t)stream, grad_grid_cap(dev), P.owner, P.w.slope, P.part, 0};
+    order_grad_forward(P, L);
+    irbpp_order_grad_head_backward_kernel<<<B, GR_THREADS, 0, L.s>>>(P);
+    // Each in-place DGRAD below overwrites an activation after the last GEMM that reads it.
+    GemmArgs g = L.base();
+    L.first(g, R);
+    L.wgrad(g, P.dadv, AC_MAXATOMS, atoms, P.ha, AC_EMB, AC_EMB, d.fc_z_a_w, AC_EMB, d.fc_z_a_b);             // fc_z_a
+    L.dgrad(g, P.dadv, AC_MAXATOMS, atoms, w.fc_z_a_w, AC_EMB, AC_EMB, P.ha, AC_EMB, ACT_RELU);              // ha <- d pre fc_h_a
+    L.wgrad(g, P.ha, AC_EMB, AC_EMB, P.h2, AC_EMB, AC_EMB, d.fc_h_a_w, AC_EMB, d.fc_h_a_b);                  // fc_h_a
+    L.dgrad(g, P.ha, AC_EMB, AC_EMB, w.fc_h_a_w, AC_EMB, AC_EMB, P.h2, AC_EMB, ACT_NONE, P.dg, AC_EMB);      // h2 <- d h2
+    L.wgrad(g, P.h2, AC_EMB, AC_EMB, P.f1, AC_EMB, AC_EMB, d.ff2_w, AC_EMB, d.ff2_b);                        // FFN.2
+    L.dgrad(g, P.h2, AC_EMB, AC_EMB, w.ff2_w, AC_EMB, AC_EMB, P.f1, AC_EMB, ACT_RELU);                       // f1 <- d pre f1
+    L.wgrad(g, P.f1, AC_EMB, AC_EMB, P.h1, AC_EMB, AC_EMB, d.ff1_w, AC_EMB, d.ff1_b);                        // FFN.0
+    L.dgrad(g, P.f1, AC_EMB, AC_EMB, w.ff1_w, AC_EMB, AC_EMB, P.h1, AC_EMB, ACT_NONE);
+    order_grad_add(P.h1, P.h2, (int64_t)R * AC_EMB, L);                                                      // h1 <- d h1
+    L.wgrad(g, P.h1, AC_EMB, AC_EMB, P.heads, AC_EMB, AC_EMB, d.wo_w, AC_EMB, d.wo_b);                      // W_out
+    L.dgrad(g, P.h1, AC_EMB, AC_EMB, w.wo_w, AC_EMB, AC_EMB, P.heads, AC_EMB, ACT_NONE);                    // heads <- d heads
+    irbpp_order_grad_attn_backward_kernel<<<B, GR_THREADS, 0, L.s>>>(P);                                     // d Q | K | V
+    float* dw[] = {d.wq, d.wk, d.wv};
+    for (int m = 0; m < 3; ++m)
+        L.wgrad(g, P.dqkv + m * AC_EMB, 384, AC_EMB, P.h, AC_EMB, AC_EMB, dw[m], AC_EMB, nullptr);         // W_query, W_key, W_val
+    L.dgrad(g, P.dqkv, 384, 384, P.wqkv, AC_EMB, AC_EMB, P.h, AC_EMB, ACT_NONE);
+    order_grad_add(P.h, P.h1, (int64_t)R * AC_EMB, L);                                                       // h <- d h
+    L.wgrad(g, P.h, AC_EMB, AC_EMB, P.p0, AC_PROJ, AC_PROJ, d.gat2_w, AC_PROJ, d.gat2_b);                   // gat_project_layer.2
+    L.dgrad(g, P.h, AC_EMB, AC_EMB, w.gat2_w, AC_PROJ, AC_PROJ, P.p0, AC_PROJ, ACT_LEAKY);                  // p0 <- d pre0
+    irbpp_order_grad_rank_kernel<<<(R + GR_THREADS - 1) / GR_THREADS, GR_THREADS, 0, L.s>>>(P);
+    irbpp_order_grad_segsum_kernel<<<S + B, GR_THREADS, 0, L.s>>>(P);                                       // Sid, Sb
+    L.first(g, S);                                                                                           // gat_project_layer.0
+    L.wgrad(g, P.Sid, AC_PROJ, AC_PROJ, P.shape_features, AC_EMB, AC_EMB, d.gat1_w, 384, nullptr);
+    L.dgrad(g, P.Sid, AC_PROJ, AC_PROJ, w.gat1_w, 384, AC_EMB, d_shape_features, AC_EMB, ACT_NONE);
+    L.first(g, B);
+    L.wgrad(g, P.Sb, AC_PROJ, AC_PROJ, P.map_feature, 256, 256, d.gat1_w + AC_EMB, 384, d.gat1_b);
+    L.dgrad(g, P.Sb, AC_PROJ, AC_PROJ, w.gat1_w + AC_EMB, 384, 256, d_map_feature, 256, ACT_NONE);
+    L.wgrad(g, P.dq, AC_MAXATOMS, atoms, P.hv, AC_EMB, AC_EMB, d.fc_z_v_w, AC_EMB, d.fc_z_v_b);              // fc_z_v
+    L.wgrad(g, P.dhv, AC_EMB, AC_EMB, P.gv, AC_EMB, AC_EMB, d.fc_h_v_w, AC_EMB, d.fc_h_v_b);                 // fc_h_v
     return launch_status();
 }
 

@@ -17,8 +17,8 @@ iteration rate.  This module keeps the loop's shape and removes the per-environm
 * ``PrioritizedReplayBank`` -- the reference's replay itself (``memory.py``: float32 sum tree, n-step returns,
   importance weights, stratified draws) for N memories on the device (``csrc/irbpp_replay.cuh``).
 * ``device_learn``         -- ``Agent.learn`` (``agent.py:68-125``) with its two no-grad passes on the device
-  (``DeviceActor.act`` / ``.target``) and, at the location level with ``gradient="device"``, the candidate-row
-  network of the gradient pass and its backward (``DeviceActor.log_prob``); the optimiser stays in torch.
+  (``DeviceActor.act`` / ``.target``) and, with ``gradient="device"``, the gradient pass's network and its backward
+  at either level (``DeviceActor.log_prob`` / ``DeviceOrderActor.log_prob``); the optimiser stays in torch.
 
 ``ReplayBank`` samples uniformly; it exists so that the actor loop can be run end to end at N = 4096 and timed
 (``tools/actor_loop.py``).
@@ -316,10 +316,12 @@ def device_learn(agent, bank, online_actor, target_actor, gradient="torch"):
        agent.py:117-121;
     7. ``bank.update_priorities`` with the loss (agent.py:123-124).
 
-    ``gradient="device"`` (location level only) replaces step 2 with ``online_actor.log_prob(states, actions)``: the
-    candidate-row network and its backward pass run as kernels (``irbpp_dqn_log_prob``), while the encoders, the
-    NoisyLinear rebuild, the loss, ``clip_grad_norm_`` and Adam stay in torch.  ``gradient="torch"`` runs the module
-    itself; it is the only path at the order level and the reference the device path is tested against.
+    ``gradient="device"`` replaces step 2 with ``online_actor.log_prob(states, actions)`` at either level: the
+    candidate-row network (``DeviceActor``, ``irbpp_dqn_log_prob``) or the order network's per-slot layers and
+    graph attention (``DeviceOrderActor``, ``irbpp_dqn_order_log_prob``) and their backward passes run as kernels,
+    while the encoders, the NoisyLinear rebuild, the loss, ``clip_grad_norm_`` and Adam stay in torch.  An order actor
+    given states of another width (a location-level batch) raises ``ValueError`` before it is called.
+    ``gradient="torch"`` runs the module itself; it is the reference the device path is tested against.
 
     One difference from the reference: its three forward passes each draw point indices with ``np.random``
     (model.py:331, 367); here the device passes draw from the counter-based generator of their actors'
@@ -330,11 +332,12 @@ def device_learn(agent, bank, online_actor, target_actor, gradient="torch"):
     if gradient not in ("torch", "device"):
         raise ValueError("gradient must be 'torch' or 'device', got %r" % (gradient,))
     if gradient == "device" and not callable(getattr(online_actor, "log_prob", None)):
-        raise ValueError("gradient='device' supports the location level (DeviceActor.log_prob); %s has no log_prob"
-                         % type(online_actor).__name__)
+        raise ValueError("gradient='device' supports the location level (DeviceActor.log_prob) and the order level "
+                         "(DeviceOrderActor.log_prob); %s has no log_prob" % type(online_actor).__name__)
     idxs, states, actions, returns, next_states, nonterminals, weights, mem_ids = bank.sample(agent.batch_size)
     B = states.shape[0]
     if gradient == "device":
+        _check_level(online_actor, states.shape[-1])
         log_ps_a = online_actor.log_prob(states, actions)
     else:
         log_ps = agent.online_net(states, log=True)
@@ -351,3 +354,12 @@ def device_learn(agent, bank, online_actor, target_actor, gradient="torch"):
     agent.optimiser.step()
     bank.update_priorities(idxs, mem_ids, loss.detach())
     return loss
+
+
+def _check_level(online_actor, width):
+    """``ValueError`` when a ``DeviceOrderActor`` is given observations of ``width`` values that are not the order
+    level's ``bufferSize + 1024`` (2 <= bufferSize <= 32); a location actor checks its own states in ``log_prob``."""
+    from .actor import HM, MAX_BUFFER, DeviceOrderActor
+    if isinstance(online_actor, DeviceOrderActor) and not 2 <= width - HM * HM <= MAX_BUFFER:
+        raise ValueError("the sampled states have %d values, not an order observation (bufferSize + 1024); a "
+                         "location-level batch needs a DeviceActor" % width)

@@ -149,10 +149,9 @@ class OrderShapeClouds(object):
         self.counter = 0                    # acts served so far
         self._epoch, self._sub = None, None
 
-    def features(self, obs_or_ids, encoder, counter=None):
-        """``DeviceShapeClouds.features`` on the current subsample: float32 ``[B, 128]``."""
+    def _subsample(self, c):
+        """The ``DeviceShapeClouds`` of act ``c``'s subsample epoch (redrawn when the epoch changes)."""
         torch = self.clouds._torch
-        c = self.counter if counter is None else int(counter)
         epoch = c // ORDER_REDRAW
         if epoch != self._epoch:
             src = self.clouds
@@ -160,7 +159,22 @@ class OrderShapeClouds(object):
             self._sub = DeviceShapeClouds(src.shape_array[:, torch.as_tensor(idx, device=src.device)], device=src.device,
                                           n_points=src.n_points, seed=src.seed, item_col=src.item_col)
             self._epoch = epoch
-        out = self._sub.features(obs_or_ids, encoder, counter=c)
+        return self._sub
+
+    def features(self, obs_or_ids, encoder, counter=None):
+        """``DeviceShapeClouds.features`` on the current subsample: float32 ``[B, 128]``."""
+        c = self.counter if counter is None else int(counter)
+        out = self._subsample(c).features(obs_or_ids, encoder, counter=c)
+        if counter is None:
+            self.counter += 1
+        return out
+
+    def sample(self, obs_or_ids, counter=None):
+        """``DeviceShapeClouds.sample`` on the current subsample: float32 ``[B, n_points, 3]``, exactly the points
+        ``features`` encodes for the same counter (``order_point_indices``), so that a module's own shape encoder can
+        be trained on them."""
+        c = self.counter if counter is None else int(counter)
+        out = self._subsample(c).sample(obs_or_ids, counter=c)
         if counter is None:
             self.counter += 1
         return out

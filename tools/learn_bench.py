@@ -11,11 +11,12 @@ forward and torch expressions), cudnn off, except for where the clouds come from
 ``shapeArray[ids]`` on the host in each of its three forward passes, which is not timed here; ``DeviceShapeClouds``
 gathers the same clouds on the device instead.  The device arm is ``device_learn``: the same gradient pass, the online
 argmax through ``DeviceActor.act`` / ``DeviceOrderActor.act`` and the target through ``.target``.  Both arms share the
-bank, start from the same weights and step their own copies.  At the location level a third arm,
-``device_grad``, is ``device_learn(..., gradient="device")``: the device arm with the gradient pass through
-``DeviceActor.log_prob`` (the candidate-row network and its backward as kernels).  The ``*_enc`` arms repeat
-``device_grad`` (location) and ``device`` (order) with ``DeviceHeightEncoder`` swapped into the online net, so the
-height encoder and its backward pass run as kernels too.
+bank, start from the same weights and step their own copies.  A third arm, ``device_grad``, is
+``device_learn(..., gradient="device")``: the device arm with the gradient pass through ``DeviceActor.log_prob``
+(the candidate-row network and its backward as kernels) or ``DeviceOrderActor.log_prob`` (the order network's
+per-slot layers, graph attention and heads and their backward as kernels).  The ``*_enc`` arms repeat
+``device_grad`` (both levels) and ``device`` (order) with ``DeviceHeightEncoder`` swapped into the online net, so the
+height encoder and its backward pass run as kernels too.  ``--levels order`` runs the order workload only.
 
 Prints one JSON line per workload: ms per call and per part (sample, gradient pass, target = online argmax + target
 pass + projection, step = loss + backward + clip + Adam, priority update) from CUDA events, medians and minima over
@@ -26,7 +27,11 @@ the same run.
 Before those, one JSON line per batch size for the height encoder alone (``bench: height_encoder``): the forward pass at
 B = 4096 (an act over 4096 bins) and forward + backward at B = 64 and 512, ``DeviceHeightEncoder`` against torch
 float32 (TF32 off) with cudnn off, as the reference trains, and with cudnn on; median and minimum ms per call from
-CUDA events.  ``--encoder-only`` prints only these lines."""
+CUDA events.  ``--encoder-only`` prints only these lines.
+
+``--profile DIR`` instead profiles one arm (``--profile-arm``, default the order level's ``device_grad_enc``) in a run of
+its own: ``torch.profiler`` with CUDA activities over ``--reps`` learns after ``--warmup``, one JSON line with the CUDA
+time per call of the gradient pass's kernels and of the whole learn, grouped by kernel name, and the trace under DIR."""
 import argparse
 import copy
 import json
@@ -149,13 +154,14 @@ def run(name, level, lib, a, dev):
     support = torch.linspace(V_MIN, V_MAX, ATOMS, device=dev)
     arms = {"torch": Arm(online, target, clouds, support, False, level),
             "device": Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level)}
-    if level == "location":
-        arms["device_grad"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True)
-        arms["device_grad_enc"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True,
-                                      True)
-    else:
+    if level == "order":
         arms["device_enc"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, False,
                                  True)
+    arms["device_grad"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True)
+    arms["device_grad_enc"] = Arm(copy.deepcopy(online), copy.deepcopy(target), clouds, support, True, level, True,
+                                  True)
+    if a.profile:
+        return profile(name, arms[a.profile_arm], bank, a)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
     times = {n: [] for n in arms}
     for i in range(a.warmup + a.reps):
@@ -175,6 +181,32 @@ def run(name, level, lib, a, dev):
         out[n]["ms_min_parts"] = {p: float(ts_p) for p, ts_p in zip(PARTS, np.array(ts).min(0))}
     out["grad_pass_share_of_device_learn"] = out["device"]["parts_ms_median"]["grad_pass"] / out["device"]["ms_median"]
     out["card"] = card()
+    print(json.dumps(out))
+
+
+def profile(name, arm, bank, a):
+    """CUDA time per learn by kernel name, from torch.profiler (a run of its own: tracing slows the host)."""
+    from torch.profiler import ProfilerActivity, profile as torch_profile
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)]
+    for _ in range(a.warmup):
+        arm.learn(bank, a.batch, ev)
+    os.makedirs(a.profile, exist_ok=True)
+    with torch_profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        for _ in range(a.reps):
+            arm.learn(bank, a.batch, ev)
+    prof.export_chrome_trace(os.path.join(a.profile, "learn_%s_%s.pt.trace.json" % (name, a.profile_arm)))
+    rows = []
+    for e in prof.key_averages():
+        us = getattr(e, "self_device_time_total", None)
+        if us is None:
+            us = e.self_cuda_time_total
+        if us > 0 and e.device_type == torch.autograd.DeviceType.CUDA:
+            rows.append((e.key, e.count / a.reps, us / 1000.0 / a.reps))
+    rows.sort(key=lambda r: -r[2])
+    out = {"profile": name, "arm": a.profile_arm, "batch": a.batch, "reps": a.reps,
+           "cuda_ms_per_learn": sum(r[2] for r in rows), "launches_per_learn": sum(r[1] for r in rows),
+           "kernels": [{"name": k[:90], "per_learn": c, "ms_per_learn": ms} for k, c, ms in rows[:40]],
+           "card": card()}
     print(json.dumps(out))
 
 
@@ -229,15 +261,24 @@ def main():
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--encoder-only", action="store_true")
+    ap.add_argument("--levels", default="location,order")
+    ap.add_argument("--profile", default=None, help="profile one arm instead, trace under this directory")
+    ap.add_argument("--profile-arm", default="device_grad_enc")
     a = ap.parse_args()
     torch.backends.cudnn.enabled = False
     dev = torch.device("cuda:0")
-    encoder_bench(a, dev)
+    levels = a.levels.split(",")
+    if a.profile:
+        levels = ["order"]
+    elif "location" in levels:
+        encoder_bench(a, dev)
     if a.encoder_only:
         return
-    run("blockout", "location", shapes.make_blockout_library(32, seed=1), a, dev)
-    run("general", "location", shapes.make_irregular_library(16, seed=2, num_rotations=8), a, dev)
-    run("blockout_buffered", "order", shapes.make_blockout_library(32, seed=1), a, dev)
+    if "location" in levels:
+        run("blockout", "location", shapes.make_blockout_library(32, seed=1), a, dev)
+        run("general", "location", shapes.make_irregular_library(16, seed=2, num_rotations=8), a, dev)
+    if "order" in levels:
+        run("blockout_buffered", "order", shapes.make_blockout_library(32, seed=1), a, dev)
 
 
 if __name__ == "__main__":
