@@ -1,7 +1,7 @@
 // irbpp.cu -- C-ABI (include/irbpp.h) host side: state ownership, table preprocessing, launches.
 //
 // No CPU fallback lives here: every entry point that computes anything launches the CUDA kernels of
-// irbpp_kernels.cuh (irbpp_scan_kernel -> irbpp_candidates_kernel).
+// irbpp_kernels.cuh (irbpp_scan_kernel or irbpp_scan_warp_kernel -> irbpp_candidates_kernel).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdarg.h>
@@ -36,6 +36,7 @@ struct irbpp_env {
     irbpp_config cfg;
     Params P;                      // device pointers + configuration (mode/inputs filled per launch)
     int scan_smem = 0;
+    int scan_warp_smem = 0;        // > 0: the online step scans with irbpp_scan_warp_kernel (block-form library, 16x16 grid)
     uint32_t* ready_dev = nullptr;       // scan -> candidates hand-over flags (one per unit)
     uint32_t epoch = 0;                  // launch counter behind the flags
     int epc = ENVS_PER_CTA_NARROW;       // bins per CTA of the candidates kernel (envs_per_cta_for(R))
@@ -164,6 +165,7 @@ static void free_dev(irbpp_env* h, void* p) {
 // `traj`: the trajectory item source, and the candidates kernel's dynamic shared memory at R rotations.
 struct StepKernels {
     void (*scan)(const Params);
+    void (*scan_warp)(const Params);     // one warp per bin: online step of a block-form library (16x16 grid only, else null)
     void (*cand)(const Params);
     void (*levels)(const Params);
     void (*heur)(const Params);
@@ -172,7 +174,9 @@ struct StepKernels {
 
 template <int EPC, class G>
 static StepKernels step_kernels_epc(bool traj, int R) {
-    return {traj ? irbpp_scan_kernel<G, true> : irbpp_scan_kernel<G, false>,
+    void (*scan_warp)(const Params) = nullptr;
+    if constexpr (G::STEP == 2) scan_warp = traj ? irbpp_scan_warp_kernel<true> : irbpp_scan_warp_kernel<false>;
+    return {traj ? irbpp_scan_kernel<G, true> : irbpp_scan_kernel<G, false>, scan_warp,
             traj ? irbpp_candidates_kernel<EPC, G, true> : irbpp_candidates_kernel<EPC, G, false>,
             irbpp_levels_kernel<G>, irbpp_heuristic_kernel<G>, cand_smem_bytes<EPC, G>(R)};
 }
@@ -465,8 +469,17 @@ int irbpp_load_shapes(irbpp_handle h, int32_t S, int32_t R, const int32_t* dims,
     h->P.maxwh = max_entries;
     // per-warp staging lists, then the bin's candidate table row (bulk-copied by the scan kernel)
     h->scan_smem = CTA_WARPS * h->P.maxwh * (int)sizeof(TileEntry) + ((h->P.cand_stride * 2 + 15) & ~15);
-    for (bool traj : {false, true})
-        CUDA_TRY(h, raise_dynamic_smem(c.device, (const void*)step_kernels(step, h->epc, traj, h->P.R).scan, h->scan_smem));
+    // the one-warp-per-bin scan serves the online step when every table is in block form and its per-warp staging (headers of
+    // the placed item + the largest scan list) fits what the kernel's residency is built for
+    bool block_form = step == 2;
+    for (size_t i = 0; i < srot.size(); ++i) block_form = block_form && srot[i].tile > 1;
+    const int warp_bytes = scanw_warp_bytes(R, max_entries);
+    h->scan_warp_smem = (block_form && h->P.K == 1 && warp_bytes <= SCANW_WARP_DYN_MAX) ? CTA_WARPS * warp_bytes : 0;
+    for (bool traj : {false, true}) {
+        const StepKernels k = step_kernels(step, h->epc, traj, h->P.R);
+        CUDA_TRY(h, raise_dynamic_smem(c.device, (const void*)k.scan, h->scan_smem));
+        if (h->scan_warp_smem) CUDA_TRY(h, raise_dynamic_smem(c.device, (const void*)k.scan_warp, h->scan_warp_smem));
+    }
     h->shapes_loaded = true;
     return IRBPP_OK;
 }
@@ -611,6 +624,9 @@ static int launch(irbpp_env* h, Params& P, cudaStream_t s) {
     if (P.mode == MODE_DEBUG_HULLS) {
         void (*levels)(const Params) = k.levels;
         levels<<<P.N, CTA_THREADS, 0, s>>>(P);
+    } else if (P.mode == MODE_STEP && h->scan_warp_smem) {
+        void (*scan)(const Params) = k.scan_warp;
+        scan<<<(units + CTA_WARPS - 1) / CTA_WARPS, CTA_THREADS, h->scan_warp_smem, s>>>(P);
     } else {
         void (*scan)(const Params) = k.scan;
         scan<<<units, CTA_THREADS, h->scan_smem, s>>>(P);

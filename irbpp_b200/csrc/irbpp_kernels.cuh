@@ -11,6 +11,8 @@
 //        floor_divide semantics (cvTools.py:78-79); one Ax x Ay bitmap per (rotation, level) by warp
 //        ballots -> global scratch (L2 resident).  Tables that are constant on square blocks of cells
 //        (voxel shapes) are scanned from block maxima of the heightmap (TileEntry lists)
+//   irbpp_scan_warp_kernel   A and B of the online step for libraries whose every table is in block form (BlockOut), 16x16
+//                            grid: one warp per bin, four bins per CTA, no block barrier
 //   irbpp_candidates_kernel  one CTA per 4 bins (up to seven rotations) or 8 bins (from R = 8), one warp per bin
 //     C  candidate extraction (cvTools.py:61-103): the (bin, rotation, level) images of the CTA are
 //        ordered by a cost key; every (image, start pixel) pair is one lane's task, dealt in that order
@@ -85,6 +87,7 @@ constexpr int MAX_LEVELS = 64;           // level-image slots per (bin, rotation
 constexpr int TASKS_PER_LANE = 2;        // micro-tasks a lane takes per batch of the candidates kernel (one follow / sort / approximate cycle)
 constexpr int SCAN_MIN_CTAS = 8;         // scan CTAs per SM the scan kernel is built for (64 registers per thread)
 constexpr int SCAN_MIN_CTAS_FINE = 6;    // the same on the 32x32 grid (80 registers: with 64 the dense scan's 32 poses per lane spill)
+constexpr int SM90_SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;   // shared memory of an sm_90 SM, and what the hardware reserves per CTA
 constexpr int TASK_TAB = 384;            // start pixels of a round listed explicitly (the rest are found by search)
 constexpr int FAST_CAP = 64;             // contour points on the fast path (32 was measured slower: every overflow redo stalls a warp)
 constexpr int LEVEL_OFFSET = 32;         // levels in [-32, 31] -> presence bit (level + 32)
@@ -250,9 +253,10 @@ __device__ __forceinline__ void store_error(const Params& P, int env, int err) {
 // cell (x, y) of a bin's heightmap in the column-parity planes: [y & 1][x][y >> 1]
 __host__ __device__ __forceinline__ int hm_index(int x, int y) { return ((y & 1) * HX + x) * (HY / 2) + (y >> 1); }
 
-// all threads of a CTA: zero one bin's heightmap (8 KB, shared or global memory) with 16-byte stores
-__device__ __forceinline__ void zero_heightmap(double* hm) {
-    for (int i = threadIdx.x; i < HX * HY / 2; i += CTA_THREADS) reinterpret_cast<double2*>(hm)[i] = make_double2(0.0, 0.0);
+// all threads of a CTA (or the `nthreads` threads numbered by `t`): zero one bin's heightmap (8 KB, shared or global
+// memory) with 16-byte stores
+__device__ __forceinline__ void zero_heightmap(double* hm, int t = threadIdx.x, int nthreads = CTA_THREADS) {
+    for (int i = t; i < HX * HY / 2; i += nthreads) reinterpret_cast<double2*>(hm)[i] = make_double2(0.0, 0.0);
 }
 
 // splitmix64 of (seed, env, draw counter): the 64-bit value behind the counter-based item sources
@@ -329,6 +333,16 @@ __device__ __forceinline__ bool env_idle(const Params& P, int env) {
 // items in a bin's queue, what reset() fills: buffer_size, one for the online setting (K = 1)
 __host__ __device__ __forceinline__ int queue_len(int K) { return K > 1 ? K : 1; }
 
+// reset and auto-reset (reset(), binPhy.py), one thread: clear the episode counters, start the next trajectory (bounds
+// `b`, `e` as for begin_trajectory) and fill the queue; false when the bin has no trajectory left (it turns idle)
+template <bool TRAJ>
+__device__ __forceinline__ bool start_episode(const Params& P, int env, EnvState& st, int& next, int& err, int64_t b, int64_t e) {
+    st.packed = 0; st.ep_len = 0; st.vol_sum = 0.0; st.ep_rew = 0.0; st.order_act = 0;
+    const bool live = !TRAJ || begin_trajectory(P, st, next, b, e);
+    if (live) for (int q = 0; q < queue_len(P.K); ++q) st.queue[q] = draw_item<TRAJ>(P, env, st, next, err);
+    return live;
+}
+
 __host__ __device__ __forceinline__ bool mode_emits_loc(int mode, int K) {
     return !((mode == MODE_STEP || mode == MODE_RESET) && K > 1);
 }
@@ -361,21 +375,25 @@ __device__ __forceinline__ void bucket_prefix64(const int32_t* hist, int32_t* hb
     hbase[32 + lane] = tot0 + i1 - h1;
 }
 
-// Per-phase SM cycles (irbpp_debug_phase_cycles): thread 0 of a CTA adds the cycles since its previous mark to counter `idx`.
-// `t` holds thread 0's previous mark; the scan kernel keeps it in shared memory, so that no thread carries it in registers
+// Per-phase SM cycles (irbpp_debug_phase_cycles): thread 0 of a CTA (PER_WARP: lane 0 of every warp, the one-warp-per-bin
+// scan) adds the cycles since its previous mark to counter `idx`.
+// `t` holds that thread's previous mark; the scan kernels keep it in shared memory, so that no thread carries it in registers
 // through phase B.
-struct PhaseClock {
+template <bool PER_WARP>
+struct PhaseClockT {
     const Params& P;
     long long& t_prev;
-    __device__ __forceinline__ PhaseClock(const Params& p, long long& t) : P(p), t_prev(t) { if (P.phase_cycles && threadIdx.x == 0) t_prev = clock64(); }
+    __device__ __forceinline__ static bool lead() { return PER_WARP ? (threadIdx.x & 31) == 0 : threadIdx.x == 0; }
+    __device__ __forceinline__ PhaseClockT(const Params& p, long long& t) : P(p), t_prev(t) { if (P.phase_cycles && lead()) t_prev = clock64(); }
     __device__ __forceinline__ void mark(int idx) {
-        if (P.phase_cycles && threadIdx.x == 0) {
+        if (P.phase_cycles && lead()) {
             const long long now = clock64();
             atomicAdd(P.phase_cycles + idx, (unsigned long long)(now - t_prev));
             t_prev = now;
         }
     }
 };
+using PhaseClock = PhaseClockT<false>;
 
 // ---- level images of one rotation -------------------------------------------------------------------
 // presence bit of level L in [-32, 31]
@@ -615,6 +633,7 @@ static inline void ready_publish(uint32_t* f, uint32_t v) { __atomic_store_n(f, 
 static inline uint32_t ready_peek(const uint32_t* f) { return __atomic_load_n(f, __ATOMIC_ACQUIRE); }
 static inline void grid_dependency_wait() {}
 static inline void backoff() {}
+static inline int opaque_zero() { return 0; }
 #else
 __device__ __forceinline__ void ready_publish(uint32_t* f, uint32_t v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(f), "r"(v) : "memory"); }
 __device__ __forceinline__ uint32_t ready_peek(const uint32_t* f) {
@@ -624,6 +643,7 @@ __device__ __forceinline__ uint32_t ready_peek(const uint32_t* f) {
 }
 __device__ __forceinline__ void grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void backoff() { __nanosleep(100); }
+__device__ __forceinline__ int opaque_zero() { int z; asm volatile("mov.u32 %0, 0;" : "=r"(z)); return z; }   // 0, unknown to the optimiser
 #endif
 constexpr int READY_POLLS = 1 << 16;       // ~10 ms of polling before the fallback
 
@@ -711,14 +731,7 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
     int next_seq = st_s.next_seq;          // thread 0's register copy; written back with the state
     int draw_err = 0;                      // thread 0: ERR_TRAJ_END of a draw past the trajectory's end
     auto draw = [&]() { return draw_item<TRAJ>(P, env, st_s, next_seq, draw_err); };
-    // thread 0, reset and auto-reset (reset(), binPhy.py): clear the episode counters, start the next trajectory and fill
-    // the queue; false when the bin has no trajectory left (it turns idle)
-    auto start_episode = [&]() {
-        st_s.packed = 0; st_s.ep_len = 0; st_s.vol_sum = 0.0; st_s.ep_rew = 0.0; st_s.order_act = 0;
-        const bool live = !TRAJ || begin_trajectory(P, st_s, next_seq, tb_pf, te_pf);
-        if (live) for (int q = 0; q < queue_len(P.K); ++q) queue_g[q] = draw();
-        return live;
-    };
+    auto start_episode = [&]() { return irbpp::start_episode<TRAJ>(P, env, st_s, next_seq, draw_err, tb_pf, te_pf); };   // thread 0
 
     // ---- phase A: bookkeeping / apply action ----
     if (idle_in) {
@@ -924,6 +937,223 @@ __global__ void __launch_bounds__(CTA_THREADS, (G::STEP == 2 ? SCAN_MIN_CTAS : S
     clock.mark(1);   // observation heightmap, write-back, scan, level bitmaps
 }
 
+// ---- one-warp-per-bin scan kernel (online step of a block-form library on the 16x16 grid) ---------------------
+// On a library whose every bottom table is in block form (tile > 1, voxel shapes such as BlockOut) phase B reads only the
+// 2x2 / 4x4 block maxima of the heightmap, and a rotation is at most 4 passes x 2 poses per lane over a short entry list.
+// irbpp_scan_kernel spends a CTA of four warps on such a bin: phase A is thread-0 and warp-0 work behind block barriers
+// while the other warps wait, and the CTA's 8 KB shared copy of the heightmap caps an SM at 8 bins.  Here one warp
+// carries a bin from the action to the hand-over without a block barrier: the drop height reads the placed window from
+// global memory, the update writes the raised cells back there, and the lanes then stream the final heightmap once to
+// write the float32 observation and take the 2x2 block maxima.  A CTA holds four bins, so an SM keeps 32 bins in flight.
+// Results, scratch and state are those irbpp_scan_kernel writes for the same call, bit for bit; the candidates kernel
+// is the same.
+// Shared memory: per warp the block maxima (2 x 2 KB), the bin's state and phase mark (static), the placed item's
+// table headers and the scan-list staging (dynamic, scanw_warp_bytes).
+struct ScanWarpSmem {
+    double p2[CTA_WARPS][Grid<2>::NPOSE];                 // 2x2 block maxima
+    double m4[CTA_WARPS][Grid<2>::NPOSE];                 // 4x4 block maxima (tile == 4)
+    EnvState st[CTA_WARPS];
+    long long t_phase[CTA_WARPS];
+    int err[CTA_WARPS];                                   // the bin's error code (lane 0)
+};
+constexpr int SCANW_WARP_DYN_MAX = 2048;                  // dynamic bytes per warp the kernel is built for (host-checked)
+__host__ __device__ constexpr int scanw_warp_bytes(int R, int maxwh) {
+    return ((R * (int)sizeof(ShapeRot) + 15) & ~15) + maxwh * (int)sizeof(TileEntry);
+}
+// 8 CTAs of 4 bins per SM: 64 registers per thread fill the register file (__launch_bounds__), and the shared memory fits
+static_assert(SCAN_MIN_CTAS * ((int)sizeof(ScanWarpSmem) + CTA_WARPS * SCANW_WARP_DYN_MAX + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM,
+              "one-warp-per-bin scan: 8 CTAs of 4 bins must fit an SM's shared memory");
+
+template <bool TRAJ>
+__global__ void __launch_bounds__(CTA_THREADS, SCAN_MIN_CTAS) irbpp_scan_warp_kernel(const Params P) {
+    using G = Grid<2>;
+    __shared__ __align__(16) ScanWarpSmem S;
+    extern __shared__ __align__(16) unsigned char scanw_dyn[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int env = P.env_lo + blockIdx.x * CTA_WARPS + warp;
+    asm volatile("griddepcontrol.launch_dependents;");      // the candidates grid may be scheduled as this one drains (PDL)
+    if (env >= P.env_hi) return;
+    PhaseClockT<true> clock(P, S.t_phase[warp]);
+    const int hdr_bytes = (P.R * (int)sizeof(ShapeRot) + 15) & ~15;
+    unsigned char* wdyn = scanw_dyn + warp * scanw_warp_bytes(P.R, P.maxwh);
+    ShapeRot* srot_w = reinterpret_cast<ShapeRot*>(wdyn);                   // headers of the placed item, all rotations
+    TileEntry* es = reinterpret_cast<TileEntry*>(wdyn + hdr_bytes);          // scan list of the rotation being scanned
+    EnvState& st = S.st[warp];
+    double* hm_g = P.hm + (int64_t)env * (HX * HY);
+
+    // ---- the bin's state and action ----
+    {
+        const uint32_t stw = reinterpret_cast<const uint32_t*>(P.state + env)[lane];
+        reinterpret_cast<uint32_t*>(&st)[lane] = stw;
+    }
+    const int64_t a = P.actions[env];
+    __syncwarp();
+    // trajectory replay: a bin with no trajectory left ignores the step (no draw, no placement, no error)
+    const bool idle_in = TRAJ && st.traj_len == TRAJ_IDLE;
+    int item = -1;                        // the next item, -1: the bin is idle
+    if (idle_in) {
+        if (lane == 0) {
+            store_results(P, env, 0.0f, 0, 0, -1, 0, -1.0, 0.0);    // reward 0, done 0, Valid 0
+            S.err[warp] = 0;
+        }
+    } else {
+        // ---- phase A: decode the action, drop height and placement test of that pose, heightmap update ----
+        int64_t tb_pf = 0, te_pf = 0;     // lane 0: bounds of the trajectory an auto-reset would start
+        if (TRAJ && lane == 0 && st.traj_next < P.traj_end) { tb_pf = P.traj_off[st.traj_next]; te_pf = P.traj_off[st.traj_next + 1]; }
+        double rew_pf = 0.0, vol_pf = 0.0;
+        if (lane == 0) { rew_pf = P.reward_tab[st.cur_item]; vol_pf = P.vol[st.cur_item]; }
+        {
+            static_assert(sizeof(ShapeRot) % 8 == 0, "headers are copied as 8-byte words");
+            constexpr int HW = (int)(sizeof(ShapeRot) / 8);
+            const unsigned long long* src = reinterpret_cast<const unsigned long long*>(P.srot + (int64_t)st.cur_item * P.R);
+            for (int i = lane; i < P.R * HW; i += 32) reinterpret_cast<unsigned long long*>(srot_w)[i] = src[i];
+        }
+        int rot = 0, lx = 0, ly = 0;
+        bool ok = true;
+        int err = 0;
+        if (a < 0 || a >= (P.pose_actions ? P.R * G::NPOSE : P.sel)) { ok = false; err = 2; }
+        else {
+            const uint32_t c = P.pose_actions ? (uint32_t)a : (uint32_t)P.cand[(int64_t)env * P.cand_stride + a];
+            rot = G::rot_of(c); lx = G::x_of(c); ly = G::y_of(c);
+            if (rot >= P.R) { rot = 0; ok = false; err = 2; }
+        }
+        __syncwarp();                     // headers visible to every lane
+        const ShapeRot& sr = srot_w[rot];
+        const int w = sr.w, h = sr.h;
+        const double* __restrict__ T = P.Ts + sr.off;
+        double tp0 = -INFINITY, tp1 = -INFINITY;          // this lane's first two cells of the top table
+        if (lane < w * h) tp0 = T[lane];
+        if (lane + 32 < w * h) tp1 = T[lane + 32];
+        // prejudge (binPhy.py:238-245)
+        if (!((sr.okx >> lx) & 1u) || !((sr.oky >> ly) & 1u)) ok = false;
+        if (!st.mask_any) ok = false;
+        double z = POSZ_INVALID;          // posZmap keeps 1e3 outside the scanned range (space.py:101)
+        if (lx < sr.nX && ly < sr.nY) {
+            const double* __restrict__ B = P.Bs + sr.off;
+            double acc = sr.any_zero ? 0.0 : -INFINITY;
+            for (int c = lane; c < w * h; c += 32) {
+                const int i = c / h, j = c - i * h;
+                const double v = hm_g[hm_index(G::STEP * lx + i, G::STEP * ly + j)] - B[c];
+                acc = (v > acc) ? v : acc;
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const double t = __shfl_xor_sync(0xffffffffu, acc, o);
+                acc = (t > acc) ? t : acc;
+            }
+            z = acc;
+        }
+        // Interface.simulateHeight (Interface.py:365-369): AABB top above the bin -> failure
+        if (ok && !round6_le0(z + sr.ez - P.binz)) ok = false;
+        if (ok) {
+            // heightmap update: hm[win] = max(hm[win], (T + z) * maskT)   (space.py:213), only the raised cells are written
+            const int x0 = G::STEP * lx, y0 = G::STEP * ly;
+            for (int c = lane; c < w * h; c += 32) {
+                const int i = c / h, j = c - i * h;
+                const double t = (c == lane) ? tp0 : ((c == lane + 32) ? tp1 : T[c]);
+                const double v = t + z;
+                const int idx = hm_index(x0 + i, y0 + j);
+                if (v > hm_g[idx]) hm_g[idx] = v;
+            }
+        } else {
+            zero_heightmap(hm_g, lane, 32);          // auto-reset
+        }
+        if (lane == 0) {
+            int next_seq = st.next_seq, draw_err = 0;
+            const int nfill = queue_len(P.K);
+            bool live = true;
+            if (ok) {
+                store_results(P, env, (float)rew_pf, 0, 1, -1, 0, -1.0, 0.0);
+                st.packed += 1; st.ep_len += 1;
+                st.vol_sum += vol_pf;
+                st.ep_rew += rew_pf;
+                // item_creator.update_item_queue(orderAction); generate_item()  (binPhy.py:324-325)
+                for (int q = st.order_act; q + 1 < nfill; ++q) st.queue[q] = st.queue[q + 1];
+                st.queue[nfill - 1] = draw_item<TRAJ>(P, env, st, next_seq, draw_err);
+            } else {
+                store_results(P, env, 0.0f, 1, 1, st.packed, st.ep_len + 1, st.vol_sum / P.binvol, st.ep_rew + 0.0);
+                live = start_episode<TRAJ>(P, env, st, next_seq, draw_err, tb_pf, te_pf);
+            }
+            st.next_seq = next_seq;
+            S.err[warp] = draw_err ? draw_err : err;
+            item = live ? st.queue[0] : -1;
+        }
+        item = __shfl_sync(0xffffffffu, item, 0);
+        __syncwarp();                     // the heightmap in global memory is final and visible to every lane
+    }
+    clock.mark(0);   // load + phase A
+
+    float* obs_g = P.obs + (int64_t)env * P.obs_stride;
+    const int ncand = P.sel * 5;
+    const bool scanned = !TRAJ || item >= 0;
+    bool any = false;
+    if (scanned) {
+        const int tile = P.srot[(int64_t)item * P.R].tile;      // same for every rotation of a shape
+        // One pass over the heightmap: lanes 0-15 take action row a = 2k, lanes 16-31 row 2k + 1, lane b of a half the
+        // four cells (2a + dx, 2b + dy) of block (a, b) -- every load of a half-warp is one 128-byte segment of a plane
+        // (even / odd y).  Each lane writes its cells to the observation (row-major x * 32 + y) and the block's maximum.
+        float* obs_hm = obs_g + ncand + 9;
+        double* p2 = S.p2[warp];
+        const int b = lane & 15;
+#pragma unroll 2
+        for (int k = 0; k < G::AX / 2; ++k) {
+            const int ra = 2 * k + (lane >> 4);
+            const double* p0 = hm_g + (2 * ra) * (HY / 2) + b;                 // plane of even y, row x = 2a
+            const double* p1 = p0 + HX * (HY / 2);                              // plane of odd y
+            const double e0 = p0[0], e1 = p0[HY / 2], o0 = p1[0], o1 = p1[HY / 2];
+            float* q = obs_hm + (2 * ra) * HY + 2 * b;
+            q[0] = (float)e0; q[1] = (float)o0; q[HY] = (float)e1; q[HY + 1] = (float)o1;
+            const double m0 = (e0 > e1) ? e0 : e1;
+            const double m1 = (o0 > o1) ? o0 : o1;
+            p2[ra * G::AY + b] = (m0 > m1) ? m0 : m1;
+        }
+        if (lane < 9) obs_g[ncand + lane] = (lane == 0) ? (float)item : 0.0f;      // next_item_vec (binPhy.py:191)
+        __syncwarp();
+        const double* Marr = p2;
+        if (tile == 4) {
+            double* m4 = S.m4[warp];
+            for (int e = lane; e < G::NPOSE; e += 32) {
+                double m = -INFINITY;
+                if ((e >> 4) < G::AX - 1 && (e & 15) < G::AY - 1) {
+                    const double m0 = (p2[e] > p2[e + 1]) ? p2[e] : p2[e + 1];
+                    const double m1 = (p2[e + 16] > p2[e + 17]) ? p2[e + 16] : p2[e + 17];
+                    m = (m0 > m1) ? m0 : m1;
+                }
+                m4[e] = m;
+            }
+            __syncwarp();
+            Marr = m4;
+        }
+        // ---- phase B: every rotation of the next item ----
+        // (the zero offset is opaque to the compiler: hoisted out of the loop, the pose addresses of all four passes stay
+        // live across the rotations and spill at 64 registers)
+        int serr = 0;
+        for (int r = 0; r < P.R; ++r) {
+            any |= scan_rotation(P, Marr + opaque_zero(), 16, es, env, item, r, lane, serr);
+        }
+        if (__any_sync(0xffffffffu, serr) && lane == 0) S.err[warp] = 4;
+    } else {
+        // an all-zero observation row (no valid candidate); the candidates kernel skips the bin
+        for (int i = lane; i < P.loc_len; i += 32) obs_g[i] = 0.0f;
+    }
+
+    // ---- the one exit: error code, state write-back, hand-over flag ----
+    if (lane == 0) {
+        store_error(P, env, S.err[warp]);
+        if (scanned) { st.cur_item = item; st.mask_any = any; }     // a bin that turned idle keeps them
+    }
+    __syncwarp();
+    reinterpret_cast<uint32_t*>(P.state + env)[lane] = reinterpret_cast<const uint32_t*>(&st)[lane];
+    if (P.ready) {
+        // hand-over: every write of the warp (scratch, observation, state) happens-before lane 0's release store through
+        // the warp barrier -- bar.warp.sync orders the memory accesses of the lanes it joins as bar.sync does a CTA's, and
+        // a release is cumulative over what its thread has synchronised with -- so one fence per bin is enough
+        __syncwarp();
+        if (lane == 0) ready_publish(P.ready + env, P.epoch);
+    }
+    clock.mark(1);   // observation heightmap, block maxima, write-back, scan, level bitmaps
+}
+
 
 // ---- levels kernel (MODE_DEBUG_HULLS): level bitmaps from caller-supplied posZValid / mask ------------------
 template <class G>
@@ -1091,7 +1321,6 @@ __host__ __device__ constexpr int cand_smem_bytes(int R) {
 // the hardware reserves 1 KB per CTA.
 template <int EPC, class G>
 __host__ __device__ constexpr int cand_min_ctas() { return (G::STEP == 2 ? 32 : 16) / EPC; }
-constexpr int SM90_SMEM_PER_SM = 228 * 1024, SMEM_RESERVED_PER_CTA = 1024;
 template <class G>
 constexpr bool cand_smem_fits() {
     return cand_min_ctas<ENVS_PER_CTA_NARROW, G>() * (cand_smem_bytes<ENVS_PER_CTA_NARROW, G>(WIDE_MIN_R - 1) + SMEM_RESERVED_PER_CTA) <= SM90_SMEM_PER_SM &&

@@ -15,6 +15,7 @@ sys.path.insert(0, ROOT)
 import test_kernels_emulated as t  # noqa: E402
 import test_narrow_spill  # noqa: E402
 import test_item_sources  # noqa: E402
+import test_scan_warp  # noqa: E402
 
 emu = t.build_emulated(tempfile.mkdtemp(), defs=sys.argv[1:] + ["-fsanitize=address", "-g", "-fno-omit-frame-pointer"])
 test_narrow_spill.test_emulated_narrow_shape_list_spill(emu); print("narrow-shape list spill ok")
@@ -32,3 +33,5 @@ for tag in ("blockout", "irregular", "cube"):
 for name, steps in (("episode_blockout", 12), ("episode_irregular", 4), ("episode_truncate", 4), ("episode_buffered", 5),
                     ("episode_rot24", 2)):
     t._replay(emu, name, steps); print(name, "ok")
+for edge, steps in ((0.08, 14), (0.02, 3)):
+    test_scan_warp.test_emulated_warp_scan_episodes_and_invalid_actions(emu, edge, steps); print("warp scan edge", edge, "ok")
